@@ -177,3 +177,62 @@ def test_tc_stream_k_grouped_heads(cuda_device, M, N, K):
             got = out[:, i * N:(i + 1) * N].float()
             assert (got - ref).abs().max().item() <= 2e-2 * max(1.0, ref.abs().max().item())
         assert int(sync.abs().sum()) == 0
+
+
+@pytest.mark.parametrize("M", [1000, 16000])
+def test_tc_backward_dx_shapes(cuda_device, M):
+    """The forward kernel at the shapes the training backward uses it for (dX = dZ W^T), with
+    bias = NULL and no ReLU, bf16 stores within the derived bound of test_train_backward_gpu:
+      head 1   (M, 992, 1920), ldo = 1024: the last N tile is 224 wide; columns 984..991 come
+               from the zero pad rows of W^T, 992..1023 must keep their sentinel;
+      layer 2  grouped (M, 640, 256) x 3 with col_off = i * 640 into ldo = 1920;
+      layer 3  (M, 256, 128), ldo = 384: columns 256..383 keep their sentinel."""
+    from morefusion_b200 import _lib
+    from morefusion_b200.contrib.singleview_3d.models.model import GemmParams
+    from test_train_backward_gpu import F64, bf16_tol, c_mma, check, control
+    L = _lib.lib()
+    g = torch.Generator(device=cuda_device).manual_seed(M)
+    rn = lambda *s: torch.randn(*s, generator=g, device=cuda_device)     # noqa: E731
+    S = -3.0
+    # head 1
+    A = rn(M, 1920).to(torch.bfloat16)
+    W = torch.zeros(992, 1920, device=cuda_device, dtype=torch.bfloat16)
+    W[:984] = (rn(984, 1920) / 40).to(torch.bfloat16)
+    out = torch.full((M, 1024), S, device=cuda_device, dtype=torch.bfloat16)
+    assert _call("tc", A, W, None, out, M, 992, 1920, lda=1920, relu=0, ldo=1024) == 0
+    ref = A.to(F64) @ W.to(F64).T
+    tol = bf16_tol(ref, A.to(F64).abs() @ W.to(F64).abs().T, c_mma(1920))
+    check("head1 dX", out[:, :992], ref, tol)
+    assert torch.count_nonzero(out[:, 984:992]) == 0
+    assert bool((out[:, 992:] == S).all()), "columns past N written"
+    control("head1 dX / last K block dropped", out[:, :992], A[:, :1856].to(F64) @ W[:, :1856].to(F64).T, tol)
+    # layer 2: three heads grouped, column offsets into one 1920-wide row (one sentinel row below)
+    dz = rn(M, 768).to(torch.bfloat16)
+    Ws = [(rn(640, 256) / 16).to(torch.bfloat16) for _ in range(3)]
+    out = torch.full((M + 1, 1920), S, device=cuda_device, dtype=torch.bfloat16)
+    views = [dz[:, i * 256:] for i in range(3)]
+    arr = (GemmParams * 3)()
+    for i in range(3):
+        arr[i] = GemmParams(_lib.ptr(views[i]), _lib.ptr(Ws[i]), None, _lib.ptr(out), M, 640, 256,
+                            0, 768, 256, 0, 0, 0, 0, 1920, i * 640)
+    ws = torch.empty(L.mf_gemm_bf16_tc_workspace_bytes(M, 640), dtype=torch.uint8, device=cuda_device)
+    assert L.mf_gemm_bf16_tc_grouped(arr, 3, _lib.ptr(ws), ws.numel(), _lib.stream()) == 0
+    torch.cuda.synchronize()
+    for i in range(3):
+        z = dz[:, i * 256:(i + 1) * 256].to(F64)
+        ref = z @ Ws[i].to(F64).T
+        tol = bf16_tol(ref, z.abs() @ Ws[i].to(F64).abs().T, c_mma(256))
+        check(f"layer2 dX head {i}", out[:M, i * 640:(i + 1) * 640], ref, tol)
+        if i == 1:
+            control("layer2 dX / col_off + 8", out[:M, i * 640:(i + 1) * 640], torch.roll(ref, 8, 1), tol)
+    assert bool((out[M] == S).all())
+    # layer 3: K = 128 (two K blocks), ldo = 384
+    dz = rn(M, 128).to(torch.bfloat16)
+    W = (rn(256, 128) / 11).to(torch.bfloat16)
+    out = torch.full((M, 384), S, device=cuda_device, dtype=torch.bfloat16)
+    assert _call("tc", dz, W, None, out, M, 256, 128, lda=128, relu=0, ldo=384) == 0
+    ref = dz.to(F64) @ W.to(F64).T
+    tol = bf16_tol(ref, dz.to(F64).abs() @ W.to(F64).abs().T, c_mma(128))
+    check("layer3 dX", out[:, :256], ref, tol)
+    assert bool((out[:, 256:] == S).all())
+    control("layer3 dX / relu applied", out[:, :256], ref.clamp_min(0), tol)
