@@ -258,36 +258,37 @@ def test_fused_head4_and_concurrent_branches_equal_sequential(cuda_device):
 
 def test_runner_graph_equals_forward_features(cuda_device):
     """The serving entry (pinned host blob -> one H2D copy -> captured CUDA graphs -> one D2H
-    copy) returns exactly what forward_features computes for the same batch, across batches."""
+    copy) returns exactly what forward_features computes for the same batch, across batches, at
+    B = 2 and at B = 8 (the batch bench.py times through this runner)."""
     from morefusion_b200.contrib.singleview_3d.models import Model
-    B = 2
     w = ocnn.init_weights(21, seed=6)
     m = Model(n_fg_class=21, with_occupancy=True).to(cuda_device).load_reference_weights(w)
-    runner = m.make_runner(B, 1000, cuda_device, graph=True)
-    for seed in (21, 22, 23):
-        inp = make_inputs(B, seed=seed)
-        runner.load_host(inp)
-        runner.run()
-        host = runner.download()
-        torch.cuda.synchronize()
-        got = [host[k].clone() for k in ("rot", "trans", "conf")]
-        want = m.forward_features(
-            class_id=torch.as_tensor(inp["class_id"], device=cuda_device),
-            values=torch.as_tensor(inp["values"], device=cuda_device),
-            points=torch.as_tensor(inp["points"], device=cuda_device),
-            pitch=inp["pitch"], origin=inp["origin"],
-            grid_nontarget_empty=torch.as_tensor(inp["grid_nontarget_empty"], device=cuda_device))
-        torch.cuda.synchronize()
-        for a, b in zip(got, want):
-            assert torch.equal(a, b.cpu())
-        # the end-to-end graph (both copies inside, `values` copied under the occupancy branch):
-        # scribble over the device inputs and the host outputs first
-        runner.in_blob.fill_(0x55)
-        runner.host_out_blob.zero_()
-        host = runner.run_e2e()
-        torch.cuda.synchronize()
-        for k, b in zip(("rot", "trans", "conf"), want):
-            assert torch.equal(host[k], b.cpu()), k
+    for B in (2, 8):
+        runner = m.make_runner(B, 1000, cuda_device, graph=True)
+        for seed in (21, 22, 23):
+            inp = make_inputs(B, seed=seed)
+            runner.load_host(inp)
+            runner.run()
+            host = runner.download()
+            torch.cuda.synchronize()
+            got = [host[k].clone() for k in ("rot", "trans", "conf")]
+            want = m.forward_features(
+                class_id=torch.as_tensor(inp["class_id"], device=cuda_device),
+                values=torch.as_tensor(inp["values"], device=cuda_device),
+                points=torch.as_tensor(inp["points"], device=cuda_device),
+                pitch=inp["pitch"], origin=inp["origin"],
+                grid_nontarget_empty=torch.as_tensor(inp["grid_nontarget_empty"], device=cuda_device))
+            torch.cuda.synchronize()
+            for k, a, b in zip(("rot", "trans", "conf"), got, want):
+                assert torch.equal(a, b.cpu()), (B, seed, k)
+            # the end-to-end graph (both copies inside, `values` copied under the occupancy
+            # branch): scribble over the device inputs and the host outputs first
+            runner.in_blob.fill_(0x55)
+            runner.host_out_blob.zero_()
+            host = runner.run_e2e()
+            torch.cuda.synchronize()
+            for k, b in zip(("rot", "trans", "conf"), want):
+                assert torch.equal(host[k], b.cpu()), (B, seed, k, "e2e")
 
 
 @pytest.mark.parametrize("D,C,s2d", [(8, 512, 0), (8, 64, 0), (8, 48, 0), (16, 256, 0), (16, 256, 1)])
@@ -322,13 +323,13 @@ def test_interp_cl_equals_public_operator(cuda_device, D, C, s2d):
     torch.testing.assert_close(got, want, rtol=2 ** -7, atol=1e-6)
 
 
+@pytest.mark.parametrize("B", [2, 8])
 @pytest.mark.parametrize("with_occ", [True, False])
-def test_cnn_precise_mode_meets_north_star_tolerance(cuda_device, with_occ):
+def test_cnn_precise_mode_meets_north_star_tolerance(cuda_device, with_occ, B):
     """Model.precision = "bf16x3" (every GEMM operand split hi + lo, three wgmma GEMMs per
     product, fp32 everywhere else): poses within 1e-4 abs of the reference's fp32 arithmetic
     (oracle/cnn.py, bf16=False) -- north_star's R/t tolerance -- on every one of the B*P
     per-point predictions, and the bf16 throughput mode bounded against the same oracle."""
-    B = 2
     w = ocnn.init_weights(21, seed=1, with_occupancy=with_occ)
     inp = make_inputs(B)
     ref32 = ocnn.forward(w, n_fg_class=21, bf16=False, **inp)
