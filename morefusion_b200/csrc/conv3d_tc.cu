@@ -65,16 +65,18 @@ __device__ __forceinline__ long long out_row_offset(const GemmParams& p, int m) 
 // operands while the consumer warpgroups run the epilogue of the current one, and the per-CTA
 // set-up (barrier init, descriptor prefetch, pipeline fill) is paid once per SM instead of once
 // per tile -- which is what the short-K head GEMMs (2-16 K blocks per tile) are dominated by.
+// With CTA pairs (CLUSTER = 2) a unit covers m-tiles 2 mt and 2 mt + 1, one per CTA of the pair,
+// and m_tiles counts the pairs.
 struct TcSched {
   int m_tiles, n_tiles, groups, splitk, n_units;
   long long* stamps;      // profiling hook (mf_gemm_bf16_tc_ex): clock64 per role per unit, CTA 0
-  // stream-K (one group, splitk == 1): the tiles x K-blocks iteration space is cut into gridDim.x
-  // equal contiguous ranges, so every SM does the same number of K blocks whatever the tile
-  // count (256 tiles on 132 SMs would otherwise leave 3 % of the machine idle in the second
-  // wave, 64 tiles more than half of it).  A CTA whose range starts inside a tile stores that
-  // segment's raw fp32 accumulator in its workspace slot and raises its flags; the CTA that
-  // holds the tile's first K block owns the tile and adds the slots of the CTAs after it, in CTA
-  // order, in its epilogue.
+  // stream-K (one group, splitk == 1): the units x K-blocks iteration space is cut into one
+  // equal contiguous range per cluster, so every SM does the same number of K blocks whatever
+  // the tile count (256 tiles on 132 SMs would otherwise leave 3 % of the machine idle in the
+  // second wave, 64 tiles more than half of it).  A CTA whose range starts inside a tile stores
+  // that segment's raw fp32 accumulator in its workspace slot and raises its flags; the CTA that
+  // holds the tile's first K block owns the tile and adds the slots of the CTAs of its own rank
+  // in the following clusters, in order, in its epilogue.
   int streamk;
   int* sk_flags;          // [gridDim.x][8] (one word per consumer warpgroup), zero between launches
   float* sk_ws;           // [gridDim.x][128 x BLOCK_N] fp32
@@ -98,20 +100,23 @@ __device__ __forceinline__ void unit_decode(const TcSched& sc, int u, int& g, in
 struct TcSeg {
   int u, kb0, kb1;
   int partial;            // stream-K: store the raw accumulator to this CTA's slot (not the output)
-  int peer0, n_peers;     // stream-K owner: add the slots of CTAs peer0 .. peer0 + n_peers - 1
+  int peer0, n_peers;     // stream-K owner: add the slots of the CTAs of its rank in clusters
+                          // peer0 .. peer0 + n_peers - 1
 };
 
+// The schedule is dealt per cluster (cid of nc): both CTAs of a pair walk the same units and K
+// ranges, each on its own m-tile.
 struct TcSegIter {
   long long pos, hi, W;   // stream-K: position in the tiles x K-blocks space
   int u;                  // otherwise: next unit
-  __device__ __forceinline__ static long long lo_of(long long W, int c) {
-    return W * c / (int)gridDim.x;
-  }
-  __device__ __forceinline__ TcSegIter(const TcSched& sc, int kb_total) {
+  int cid, nc;
+  __device__ __forceinline__ long long lo_of(int c) const { return W * c / nc; }
+  __device__ __forceinline__ TcSegIter(const TcSched& sc, int kb_total, int cid_, int nc_)
+      : cid(cid_), nc(nc_) {
     W = (long long)sc.n_units * kb_total;
-    pos = sc.streamk ? lo_of(W, blockIdx.x) : 0;
-    hi = sc.streamk ? lo_of(W, blockIdx.x + 1) : 0;
-    u = blockIdx.x;
+    pos = sc.streamk ? lo_of(cid) : 0;
+    hi = sc.streamk ? lo_of(cid + 1) : 0;
+    u = cid;
   }
   __device__ __forceinline__ bool next(const TcSched& sc, const TcExtra& e, TcSeg& s) {
     s.partial = 0; s.peer0 = 0; s.n_peers = 0;
@@ -125,9 +130,9 @@ struct TcSegIter {
       s.partial = k0 != 0;
       if (k0 == 0 && k1 < e.kb_total) {
         const long long tile_end = (long long)(t + 1) * e.kb_total;
-        s.peer0 = blockIdx.x + 1;
+        s.peer0 = cid + 1;
         int c = s.peer0;
-        while (c < (int)gridDim.x && lo_of(W, c) < tile_end) ++c;
+        while (c < nc && lo_of(c) < tile_end) ++c;
         s.n_peers = c - s.peer0;
       }
       pos += k1 - k0;
@@ -138,7 +143,7 @@ struct TcSegIter {
     s.u = u;
     s.kb0 = split * e.kb_per_split;
     s.kb1 = min(s.kb0 + e.kb_per_split, e.kb_total);
-    u += gridDim.x;
+    u += nc;
     return true;
   }
 };
@@ -155,12 +160,13 @@ constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;
 // and r0 + 8 of the warpgroup's 64, columns 8 j + 2 (t % 4) + {0, 1} in d[4 j + 2 i + {0, 1}]
 // (i = 0 for row r0, 1 for r0 + 8).
 
-// Wait until the stream-K peers of this warpgroup have parked their partial sums
-__device__ __forceinline__ void sk_wait_peers(const int* flags, int n_peers, int* err) {
+// Wait until the stream-K peers of this warpgroup have parked their partial sums (their flag
+// words are `stride` ints apart)
+__device__ __forceinline__ void sk_wait_peers(const int* flags, int n_peers, int stride, int* err) {
   for (int pi = 0; pi < n_peers; ++pi) {
     int v = 0;
     for (long long spin = 0; spin < (1LL << 24); ++spin) {
-      asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(flags + pi * 8) : "memory");
+      asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(flags + pi * stride) : "memory");
       if (v) break;
       __nanosleep(64);
     }
@@ -168,9 +174,15 @@ __device__ __forceinline__ void sk_wait_peers(const int* flags, int n_peers, int
   }
 }
 
-template <int BLOCK_N, int STAGES>
+// CLUSTER = 2 (the convolutions): the two CTAs of a cluster take m-tiles 2 mt and 2 mt + 1 of the
+// same n-tile and K range, so they need the same W tile: each producer loads its own A box and
+// half of W (rows rank x BLOCK_N / 2 ..), multicast into the same stage of both CTAs.  A stage is
+// then written by both producers, so its empty barrier counts the consumer warpgroups of both
+// CTAs, and each consumer warpgroup releases the stage in its own CTA and in its peer.
+template <int BLOCK_N, int STAGES, int CLUSTER>
 __global__ void __launch_bounds__(TC_P_THREADS, 1)
 k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
+  static_assert(CLUSTER == 1 || CLUSTER == 2, "CTA pairs at most");
   constexpr int B_BYTES = BLOCK_N * TC_BLOCK_K * 2;
   constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
   constexpr int NR = BLOCK_N / 2;                 // accumulators per consumer thread
@@ -183,6 +195,8 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const TcExtra& e = args.e;
+  const int crank = CLUSTER == 1 ? 0 : (int)cluster_ctarank();
+  const int cid = blockIdx.x / CLUSTER, nc = gridDim.x / CLUSTER;
 
   if (threadIdx.x == 0) {
     for (int g = 0; g < sc.groups; ++g) {
@@ -192,23 +206,29 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);            // one arrival per consumer warpgroup
+      mbar_init(&empty_bar[s], 2 * CLUSTER);  // one arrival per consumer warpgroup of the cluster
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
+  // the peer multicasts into this CTA's stages and arrives on its barriers: both inits first
+  if constexpr (CLUSTER == 1) __syncthreads();
+  else cluster_sync();
 
   if (warp < 4) {
     setmaxnreg_dec<TC_PRODUCER_REGS>();
-    if (threadIdx.x != 0) return;
+    if (threadIdx.x != 0) {
+      if constexpr (CLUSTER > 1) cluster_sync();
+      return;
+    }
     // ===== TMA producer
     int kc = 0;                                        // K blocks issued so far (ring position)
     int it = 0;
-    TcSegIter iter(sc, e.kb_total);
+    TcSegIter iter(sc, e.kb_total, cid, nc);
     TcSeg seg;
     for (; iter.next(sc, e, seg); ++it) {
       int g, mt, nt, split;
       unit_decode(sc, seg.u, g, mt, nt, split);
+      mt = mt * CLUSTER + crank;
       const GemmParams& p = args.p[g];
       TC_STAMP(0);
       const int m0 = mt * TC_BLOCK_M, n0 = nt * BLOCK_N;
@@ -227,18 +247,30 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
         mbar_expect_tx(&full_bar[s], STAGE_BYTES);
         unsigned char* sa = smem + (size_t)s * STAGE_BYTES;
         unsigned char* sb = sa + TC_A_BYTES;
+        int wk = kb * TC_BLOCK_K;                      // W column of the K block
         if (p.mode == GEMM_CONV_S2D) {
-          // the 128 output voxels x 64 channels of one K block are ONE 5-D box
-          int a = kb / e.kb_per_a, c = (kb - a * e.kb_per_a) * TC_BLOCK_K;
+          // the 128 output voxels x 64 channels of one K block are ONE 5-D box.  K is walked
+          // channel block by channel block with the 8 cell offsets a innermost, so the 8
+          // overlapping boxes of a channel block are read back to back while they are in L2.
+          const int a = kb & 7, c = (kb >> 3) * TC_BLOCK_K;
+          wk = a * e.kb_per_a * TC_BLOCK_K + c;
           tma_load_5d(sa, &args.tmA[g], &full_bar[s], c, cw + (a & 1), ch + ((a >> 1) & 1),
                       cd + ((a >> 2) & 1), cb);
         } else {
-          tma_load_2d(sa, &args.tmA[g], &full_bar[s], kb * TC_BLOCK_K, m0);
+          tma_load_2d(sa, &args.tmA[g], &full_bar[s], wk, m0);
         }
-        tma_load_2d(sb, &args.tmW[g], &full_bar[s], kb * TC_BLOCK_K, n0);
+        if constexpr (CLUSTER == 1) {
+          tma_load_2d(sb, &args.tmW[g], &full_bar[s], wk, n0);
+        } else {
+          // rows [crank x BLOCK_N / 2, + BLOCK_N / 2) of the W tile, at their offset in the
+          // K-major SW128 layout (1024 B per 8 rows), into this stage of both CTAs
+          tma_load_2d_multicast(sb + crank * (B_BYTES / 2), &args.tmW[g], &full_bar[s], wk,
+                                n0 + crank * (BLOCK_N / 2), (uint16_t)0x3);
+        }
       }
       TC_STAMP(1);
     }
+    if constexpr (CLUSTER > 1) cluster_sync();
     return;
   }
 
@@ -248,12 +280,19 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
   const int r0 = (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
   const bool stamper = wg == 0 && t == 0;
   constexpr long long SLOT_FLOATS = (long long)TC_BLOCK_M * BLOCK_N;
+  // a stage is free again for the producers that write it: this CTA's, and the peer's (its half
+  // of W)
+  auto release = [&](int s) {
+    mbar_arrive(&empty_bar[s]);
+    if constexpr (CLUSTER > 1) mbar_arrive_cluster(&empty_bar[s], crank ^ 1);
+  };
   int kc = 0, it = 0;
-  TcSegIter iter(sc, e.kb_total);
+  TcSegIter iter(sc, e.kb_total, cid, nc);
   TcSeg seg;
   for (; iter.next(sc, e, seg); ++it) {
     int g, mt, nt, split;
     unit_decode(sc, seg.u, g, mt, nt, split);
+    mt = mt * CLUSTER + crank;
     if (stamper) TC_STAMP(2);
     float d[NR];
     int prev = -1;
@@ -270,12 +309,12 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
       fence_regs(d);
       // keep one K block in flight: the stage of the previous one is free once it retired
       wgmma_wait<1>();
-      if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
+      if (prev >= 0 && t == 0) release(prev);
       prev = s;
     }
     wgmma_wait<0>();
     fence_regs(d);
-    if (t == 0) mbar_arrive(&empty_bar[prev]);
+    if (t == 0) release(prev);
     if (stamper) TC_STAMP(4);
 
     const GemmParams& p = args.p[g];
@@ -297,12 +336,14 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
     }
     if (seg.n_peers > 0) {
       // the peers ran these K blocks at the START of their range, this CTA reaches the tile at
-      // the END of its own: normally no wait
-      if (t == 0) sk_wait_peers(sc.sk_flags + seg.peer0 * 8 + wg, seg.n_peers, e.err);
+      // the END of its own: normally no wait.  Peer pi is the CTA of this rank in cluster
+      // peer0 + pi.
+      const int peer_cta0 = seg.peer0 * CLUSTER + crank;
+      if (t == 0) sk_wait_peers(sc.sk_flags + peer_cta0 * 8 + wg, seg.n_peers, 8 * CLUSTER, e.err);
       wg_bar(1 + wg);
       for (int pi = 0; pi < seg.n_peers; ++pi) {
         const float2* ps = reinterpret_cast<const float2*>(
-            sc.sk_ws + (long long)(seg.peer0 + pi) * SLOT_FLOATS + (long long)wg * 64 * BLOCK_N);
+            sc.sk_ws + (long long)(peer_cta0 + pi * CLUSTER) * SLOT_FLOATS + (long long)wg * 64 * BLOCK_N);
 #pragma unroll
         for (int i = 0; i < NR / 2; ++i) {
           const float2 a = __ldcg(ps + i * 128 + t);
@@ -312,7 +353,7 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
       }
       wg_bar(1 + wg);
       if (t == 0)                 // slots consumed: re-arm the flags for the next launch
-        for (int pi = 0; pi < seg.n_peers; ++pi) sc.sk_flags[(seg.peer0 + pi) * 8 + wg] = 0;
+        for (int pi = 0; pi < seg.n_peers; ++pi) sc.sk_flags[(peer_cta0 + pi * CLUSTER) * 8 + wg] = 0;
     }
     if (stamper) TC_STAMP(5);
     const int pN = p.N, pM = p.M, prelu = p.relu, pmode = p.out_mode;
@@ -361,6 +402,8 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
     }
     if (stamper) { TC_STAMP(6); TC_STAMP(7); }
   }
+  // no CTA leaves while its peer may still multicast into it or arrive on its barriers
+  if constexpr (CLUSTER > 1) cluster_sync();
 }
 
 // ------------------------------------------------------------------ the pose heads as ONE launch
@@ -609,11 +652,62 @@ static int encode(CUtensorMap* tm, const void* base, int rank, const cuuint64_t*
 }
 
 template <int BLOCK_N, int STAGES>
+static constexpr int persistent_smem() {
+  return STAGES * (TC_A_BYTES + BLOCK_N * TC_BLOCK_K * 2) + 1024;
+}
+
+template <int BLOCK_N, int STAGES>
 static int launch_persistent(const TcArgs& args, const TcSched& sc, int n_sm, cudaStream_t stream) {
-  constexpr int smem = STAGES * (TC_A_BYTES + BLOCK_N * TC_BLOCK_K * 2) + 1024;
-  MF_ENSURE_DYN_SMEM((k_gemm_tc_persistent<BLOCK_N, STAGES>), smem);
+  constexpr int smem = persistent_smem<BLOCK_N, STAGES>();
+  MF_ENSURE_DYN_SMEM((k_gemm_tc_persistent<BLOCK_N, STAGES, 1>), smem);
   int grid = (sc.n_units < n_sm && !sc.streamk) ? sc.n_units : n_sm;
-  k_gemm_tc_persistent<BLOCK_N, STAGES><<<grid, TC_P_THREADS, smem, stream>>>(args, sc);
+  k_gemm_tc_persistent<BLOCK_N, STAGES, 1><<<grid, TC_P_THREADS, smem, stream>>>(args, sc);
+  MF_LAUNCH_CHECK();
+  return MF_OK;
+}
+
+// launch configuration of `grid` CTAs in clusters of 2 (`attr` must outlive it)
+template <int BLOCK_N, int STAGES>
+static cudaLaunchConfig_t pair_config(cudaLaunchAttribute* attr, int grid, cudaStream_t stream) {
+  attr->id = cudaLaunchAttributeClusterDimension;
+  attr->val.clusterDim.x = 2;
+  attr->val.clusterDim.y = 1;
+  attr->val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(TC_P_THREADS);
+  cfg.dynamicSmemBytes = persistent_smem<BLOCK_N, STAGES>();
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cfg;
+}
+
+// How many CTA pairs can be resident at once (one CTA per SM).  Remembered per device, as
+// MF_ENSURE_DYN_SMEM does, so that calls made while a CUDA graph is captured only read it.
+template <int BLOCK_N, int STAGES>
+static int pair_clusters(int dev, int n_sm, int* n_clusters) {
+  static int known[64];
+  MF_ENSURE_DYN_SMEM((k_gemm_tc_persistent<BLOCK_N, STAGES, 2>), (persistent_smem<BLOCK_N, STAGES>()));
+  if (dev >= 0 && dev < 64 && known[dev] > 0) {
+    *n_clusters = known[dev];
+    return MF_OK;
+  }
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg = pair_config<BLOCK_N, STAGES>(&attr, n_sm & ~1, 0);
+  MF_CUDA_TRY(cudaOccupancyMaxActiveClusters(n_clusters, k_gemm_tc_persistent<BLOCK_N, STAGES, 2>, &cfg));
+  if (dev >= 0 && dev < 64) known[dev] = *n_clusters;
+  return MF_OK;
+}
+
+// at most `n_clusters` pairs, all resident: stream-K needs every CTA on an SM at once
+template <int BLOCK_N, int STAGES>
+static int launch_persistent_pairs(const TcArgs& args, const TcSched& sc, int n_clusters,
+                                   cudaStream_t stream) {
+  const int clusters = (sc.n_units < n_clusters && !sc.streamk) ? sc.n_units : n_clusters;
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg = pair_config<BLOCK_N, STAGES>(&attr, 2 * clusters, stream);
+  MF_CUDA_TRY(cudaLaunchKernelEx(&cfg, k_gemm_tc_persistent<BLOCK_N, STAGES, 2>, args, sc));
   MF_LAUNCH_CHECK();
   return MF_OK;
 }
@@ -632,7 +726,8 @@ static int check_shape(const GemmParams& p) {
   return MF_OK;
 }
 
-static int make_maps(const GemmParams& p, int BN, CUtensorMap* tmA, CUtensorMap* tmW, int* kb_per_a) {
+// w_rows: rows of the W box (the N tile, or half of it when a CTA pair shares the tile)
+static int make_maps(const GemmParams& p, int w_rows, CUtensorMap* tmA, CUtensorMap* tmW, int* kb_per_a) {
   int rc;
   *kb_per_a = 0;
   if (p.mode == GEMM_CONV_S2D) {
@@ -658,7 +753,7 @@ static int make_maps(const GemmParams& p, int BN, CUtensorMap* tmA, CUtensorMap*
   if (rc) return rc;
   cuuint64_t dims[2] = {(cuuint64_t)p.K, (cuuint64_t)p.N};
   cuuint64_t str[1] = {(cuuint64_t)p.ldw * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)BN};
+  cuuint32_t box[2] = {64, (cuuint32_t)w_rows};
   return encode(tmW, p.W, 2, dims, str, box);
 }
 
@@ -692,9 +787,22 @@ extern "C" int mf_gemm_bf16_tc_ex(const GemmParams* hp, int n_groups, void* work
     args.p[g] = hp[g];
   }
   const int BN = (p0.N >= 256) ? 256 : 128;
+  int n_sm = 132, dev = 0;
+  MF_CUDA_TRY(cudaGetDevice(&dev));
+  MF_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+  // The convolutions run as CTA pairs sharing the W tile (their m-tile count is even: M is a
+  // multiple of Do^3 >= 512), when pairs can cover every SM; linear GEMMs (odd m-tile counts
+  // such as M = 8000) as single CTAs.
+  int cluster = 1, n_pairs = 0;
+  if (p0.mode == GEMM_CONV_S2D) {
+    int rc = BN == 256 ? pair_clusters<256, 4>(dev, n_sm, &n_pairs)
+                       : pair_clusters<128, 6>(dev, n_sm, &n_pairs);
+    if (rc) return rc;
+    if (2 * n_pairs >= (n_sm & ~1)) cluster = 2;
+  }
   args.e.kb_total = (p0.K + TC_BLOCK_K - 1) / TC_BLOCK_K;
   for (int g = 0; g < n_groups; ++g) {
-    int rc = make_maps(hp[g], BN, &args.tmA[g], &args.tmW[g], &args.e.kb_per_a);
+    int rc = make_maps(hp[g], BN / cluster, &args.tmA[g], &args.tmW[g], &args.e.kb_per_a);
     if (rc) return rc;
   }
   int maxN = p0.N;
@@ -702,9 +810,6 @@ extern "C" int mf_gemm_bf16_tc_ex(const GemmParams* hp, int n_groups, void* work
   const int m_tiles = (p0.M + TC_BLOCK_M - 1) / TC_BLOCK_M, n_tiles = (maxN + BN - 1) / BN;
   int splitk = 1;
   const int tiles = m_tiles * n_tiles * n_groups;
-  int n_sm = 132, dev = 0;
-  MF_CUDA_TRY(cudaGetDevice(&dev));
-  MF_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
   // stream-K when the caller provides the flag words and whole-tile scheduling would idle > 5 %
   // of the SMs (or there are fewer tiles than SMs) on a long-K problem with bf16 output
   bool streamk = false;
@@ -732,10 +837,16 @@ extern "C" int mf_gemm_bf16_tc_ex(const GemmParams* hp, int n_groups, void* work
     if (!workspace || workspace_bytes < (size_t)splitk * p0.M * p0.N * 4) return MF_E_WORKSPACE;
     args.e.ws = (float*)workspace;
   }
-  TcSched sc{m_tiles, n_tiles, n_groups, splitk, m_tiles * n_tiles * n_groups * splitk,
+  const int m_units = m_tiles / cluster;
+  TcSched sc{m_units, n_tiles, n_groups, splitk, m_units * n_tiles * n_groups * splitk,
              stamps, streamk ? 1 : 0, sync, (float*)workspace};
-  int rc = BN == 256 ? launch_persistent<256, 4>(args, sc, n_sm, stream)
-                     : launch_persistent<128, 6>(args, sc, n_sm, stream);
+  int rc;
+  if (cluster == 2)
+    rc = BN == 256 ? launch_persistent_pairs<256, 4>(args, sc, n_pairs, stream)
+                   : launch_persistent_pairs<128, 6>(args, sc, n_pairs, stream);
+  else
+    rc = BN == 256 ? launch_persistent<256, 4>(args, sc, n_sm, stream)
+                   : launch_persistent<128, 6>(args, sc, n_sm, stream);
   if (rc) return rc;
   if (splitk > 1) {
     MF_PREFER_MAX_SMEM(k_splitk_finish);

@@ -68,6 +68,38 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
+// ---- thread-block clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster (not .aligned: the threads of a warp may reach it from
+// different places)
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster.  Used to
+// hand a consumed stage back: what has to be ordered before it is the completion of the reads
+// of that stage (wgmma.wait_group), not memory writes, so the default .cta release suffices
+// (.release.cluster would put a GPU-wide MEMBAR in front of every arrival).
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+// one box into the same shared-memory offset of every CTA in `cta_mask`; each destination's
+// mbarrier at `bar`'s offset receives the complete_tx of the bytes that landed there
+__device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorMap* tm, uint64_t* bar,
+                                                      int c0, int c1, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
+      "h"(cta_mask)
+      : "memory");
+}
+
 // ---- wgmma (warpgroup MMA, accumulator in registers)
 // SWIZZLE_128B operand descriptor (sm_90 GMMA layout): [0,14) addr>>4 | [16,30) LBO>>4 |
 // [32,46) SBO>>4 | [62,64) layout type 1 = SWIZZLE_128B.  Stages are 1024-byte aligned, so the
