@@ -11,9 +11,9 @@
 //                 SWIZZLE_128B smem stage, mbarrier expect_tx / complete_tx
 //   warpgroups 1-2           consumers: 4 x wgmma (m64 x BLOCK_N x k16) per stage on 64 rows each,
 //                 one K block kept in flight, the stage released to the producer once its wgmma
-//                 retired; then bias, ReLU, bf16 pack and stores from the accumulator registers
-//                 (row-major, or scattered into the space-to-depth layout the next convolution's
-//                 TMA boxes read)
+//                 retired; then bias, ReLU and bf16 pack into a shared-memory staging buffer and
+//                 TMA stores (row-major, or into the space-to-depth layout the next
+//                 convolution's TMA boxes read); fp32 outputs are stored from the registers
 // For the convolutions the A operand needs no im2col: with the space-to-depth input layout
 // (cnn.cu) the 128 output voxels x 64 channels of one K block are ONE 5-D TMA box.
 #include <cuda.h>
@@ -38,13 +38,18 @@ struct TcExtra {
   int splitk;
   float* ws;         // fp32 [splitk][M][N] partial sums when splitk > 1 (plain stores, no atomics)
   int* err;          // device error word (pipeline time-out), may be null
+  int staged;        // bf16 outputs leave through the staging buffer and tmO (staged_epilogue)
 };
+
+// staging buffer of a consumer warpgroup: 64 rows x 128 columns bf16 (16 KB)
+constexpr int TC_STG_COLS = 128, TC_STG_BYTES = 64 * TC_STG_COLS * 2;
 
 constexpr int TC_MAX_GROUPS = 3;
 // up to 3 same-shape GEMMs in one launch (the three pose heads): grid.z = group * splitk + split
 struct TcArgs {
   CUtensorMap tmA[TC_MAX_GROUPS];
   CUtensorMap tmW[TC_MAX_GROUPS];
+  CUtensorMap tmO[TC_MAX_GROUPS];   // staged: row-major 2-D {N, M} or s2d 5-D output map
   GemmParams p[TC_MAX_GROUPS];
   TcExtra e;
 };
@@ -151,7 +156,7 @@ struct TcSegIter {
 
 // Warpgroup 0 produces (one thread issues the TMA loads), warpgroups 1 and 2 consume: each runs
 // wgmma on 64 of the tile's 128 rows (m64 x BLOCK_N x k16, fp32 accumulators in registers) and
-// then its own epilogue straight from those registers.
+// then its own epilogue from those registers (staged_epilogue for bf16 outputs).
 constexpr int TC_P_THREADS = 384;
 // register split between the roles (setmaxnreg): 128 x 40 + 256 x 232 <= 64 K registers per SM
 constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;
@@ -159,6 +164,136 @@ constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;
 // wgmma accumulator fragment of thread t of a consumer warpgroup: rows r0 = 16 (t / 32) + (t % 32) / 4
 // and r0 + 8 of the warpgroup's 64, columns 8 j + 2 (t % 4) + {0, 1} in d[4 j + 2 i + {0, 1}]
 // (i = 0 for row r0, 1 for r0 + 8).
+
+// ------------------------------------------------------------------ staged bf16 epilogue
+// A consumer warpgroup's 64 x BN bf16 tile goes from the accumulator fragment through its 16 KB
+// staging buffer (HC = 128 columns per pass: two 64-column slices of 8 KB) to global memory by
+// TMA stores that one thread issues; the warpgroup goes back to wgmma while they drain.  Inside a
+// slice the layout is SW128: column c of a 128-byte box row `row` sits at row x 128 +
+// ((c / 8) ^ key) x 16 + (c % 8) x 2, key = row % 8.  Where a fragment row lands in the slice and
+// which TMA stores take the slice out is the box policy's:
+//   row(k, off, key)   byte offset in the slice and SW128 key of the row the thread writes with
+//                      store k (0, 1) of a column group: fragment row r0 + 8 (k ^ swap), swap = 1
+//                      only when kSwap and the thread's r0 is odd
+//   store(slice, c0)   the stores of the slice holding output columns [c0, c0 + 64)
+
+// A row-major output (2-D map {N, M} at out + col_off, row pitch ldo, 64 x 64 boxes): fragment
+// row r is row r of the slice's one box.  The 8 row groups of a store are 8 consecutive rows, 8
+// distinct keys: no bank conflict.
+struct StgRowMajor {
+  static constexpr bool kSwap = false;
+  const CUtensorMap* tm;
+  int m0;                       // the warpgroup's first output row
+  __device__ __forceinline__ void row(int k, uint32_t& off, uint32_t& key) const {
+    const int r = (threadIdx.x >> 5 & 3) * 16 + (threadIdx.x & 31) / 4 + 8 * k;
+    off = (uint32_t)r * 128;
+    key = (uint32_t)r & 7;
+  }
+  __device__ __forceinline__ void store(uint32_t slice, int c0) const { tma_store_2d(tm, slice, c0, m0); }
+};
+
+// conv3's output scattered into the s2d layout of conv4's input x4 [B][J][J][J][8 N], J = 9:
+// padded coordinate p = o + 1 of an output voxel lands in cell p / 2 at parity slot
+// s = 4 (pd % 2) + 2 (ph % 2) + pw % 2, channels [s N, s N + N).  A warpgroup's 64 rows are 4 oh
+// (oh0 = 4 i) x 16 ow at one od, so per (ph % 2, pw % 2) they fill 2 consecutive jh x 8
+// consecutive jw cells: one box {64 channels, 8 jw, 2 jh, 1, 1} (2 KB) of a 5-D map over x4.  A
+// slice holds the 4 boxes, box (ph % 2, pw % 2) at (2 (ph % 2) + pw % 2) x 2 KB; fragment row
+// r = 16 oh_l + ow is row 8 (oh_l / 2) + ow / 2 of box (1 - oh_l % 2, 1 - ow % 2).  The zero ring
+// of x4 (p = 0 and p = 17) lies outside every box and is never written.
+// The row groups of one store are ow = 0..7 (or 8..15): even and odd ow land in two boxes at the
+// same keys ow / 2, a 2-way bank conflict.  So the threads of odd ow swap their two rows (kSwap):
+// store 0 writes ow = 0, 2, 4, 6 (keys 0-3) and 9, 11, 13, 15 (keys 4-7), store 1 the others.
+struct StgS2D {
+  static constexpr bool kSwap = true;
+  const CUtensorMap* tm;
+  int N;                        // channels per parity slot
+  int s_d, jh0, jd, b;          // pd % 2 (as slot bit 4), first jh of parity ph % 2 = 1, jd, batch
+  // Do = 16: m0 is the warpgroup's first output row (a multiple of 64)
+  __device__ __forceinline__ StgS2D(const CUtensorMap* tm_, int N_, int m0) : tm(tm_), N(N_) {
+    const int oh0 = (m0 >> 4) & 15, pd = ((m0 >> 8) & 15) + 1;
+    s_d = (pd & 1) << 2;
+    jh0 = oh0 >> 1;
+    jd = pd >> 1;
+    b = m0 >> 12;
+  }
+  __device__ __forceinline__ void row(int k, uint32_t& off, uint32_t& key) const {
+    const int oh_l = threadIdx.x >> 5 & 3, ow0 = (threadIdx.x & 31) / 4;
+    const int ow = ow0 + 8 * (k ^ (ow0 & 1));
+    const int box = 2 * (1 - (oh_l & 1)) + 1 - (ow & 1);
+    const int r = 8 * (oh_l >> 1) + (ow >> 1);
+    off = (uint32_t)(box * 2048 + r * 128);
+    key = (uint32_t)r & 7;
+  }
+  __device__ __forceinline__ void store(uint32_t slice, int c0) const {
+    if (c0 >= N) return;        // a tile wider than the slot
+#pragma unroll
+    for (int box = 0; box < 4; ++box) {
+      const int sh = box >> 1, sw = box & 1;   // ph % 2, pw % 2
+      tma_store_5d(tm, slice + box * 2048, (s_d | sh << 1 | sw) * N + c0, 1 - sw, jh0 + 1 - sh, jd, b);
+    }
+  }
+};
+
+// Bias, ReLU (folded into cvt.rn.relu) and bf16 of the warpgroup's accumulators d (fragment as
+// above, columns n0 ..), staged H = min(BN, HC) columns per pass.  Thread 0 of the warpgroup
+// waits before a pass until the stores of the previous pass have read the buffer: `first_wait()`
+// before the first pass (it may do more, as the heads' publish does), bulk_wait_read0 before the
+// others; it calls `written()` once the last pass is in shared memory, then issues that pass's
+// stores.  The stores of the last pass are left in flight (one bulk group per pass).
+template <int BN, int HC, class Boxes, class FirstWait, class Written>
+__device__ __forceinline__ void staged_epilogue(const float (&d)[BN / 2], uint32_t stg, int n0, int pN,
+                                                const float* pbias, int prelu, const Boxes& boxes,
+                                                FirstWait first_wait, Written written) {
+  constexpr int H = BN < HC ? BN : HC;        // columns per staging pass
+  const int lane = threadIdx.x & 31, t = threadIdx.x & 127, wg = (threadIdx.x >> 7) - 1;
+  const int cq = 2 * (lane & 3);
+  const bool swap = Boxes::kSwap && ((lane >> 2) & 1);
+  uint32_t off0, key0, off1, key1;
+  boxes.row(0, off0, key0);
+  boxes.row(1, off1, key1);
+  const uint32_t at0 = stg + off0 + cq * 2, at1 = stg + off1 + cq * 2;
+  // one loop over the fragment's column groups j (fully unrolled, so d[] stays in registers); a
+  // staging pass starts every H / 8 of them
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int jj = j % (H / 8);
+    if (jj == 0) {
+      if (t == 0) {
+        if (j == 0) first_wait();
+        else bulk_wait_read0();        // the staging buffer's previous stores have read it
+      }
+      wg_bar(1 + wg);
+    }
+    const int n = n0 + 8 * j + cq;
+    const bool in = n < pN;
+    const float b0 = (pbias && in) ? __ldg(pbias + n) : 0.f, b1 = (pbias && in) ? __ldg(pbias + n + 1) : 0.f;
+    uint32_t v[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const float x0 = d[4 * j + 2 * i] + b0, x1 = d[4 * j + 2 * i + 1] + b1;
+      v[i] = prelu ? pack_bf16x2_relu(x0, x1) : pack_bf16x2(x0, x1);
+    }
+    if (Boxes::kSwap) {
+      const uint32_t v0 = swap ? v[1] : v[0], v1 = swap ? v[0] : v[1];
+      v[0] = v0;
+      v[1] = v1;
+    }
+    const uint32_t sl = (uint32_t)(jj >> 3) * 8192, c = (uint32_t)jj & 7;
+    sts_b32(at0 + sl + ((c ^ key0) << 4), v[0]);
+    sts_b32(at1 + sl + ((c ^ key1) << 4), v[1]);
+    if (jj == H / 8 - 1) {
+      fence_proxy_async_smem();
+      wg_bar(1 + wg);
+      if (t == 0) {
+        if (j == BN / 8 - 1) written();
+        const int c0 = n0 + (j / (H / 8)) * H;
+#pragma unroll
+        for (int s = 0; s < H / 64; ++s) boxes.store(stg + s * 8192, c0 + 64 * s);
+        bulk_commit();
+      }
+    }
+  }
+}
 
 // Wait until the stream-K peers of this warpgroup have parked their partial sums (their flag
 // words are `stride` ints apart)
@@ -202,6 +337,8 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
     for (int g = 0; g < sc.groups; ++g) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&args.tmA[g])) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&args.tmW[g])) : "memory");
+      if (e.staged)
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&args.tmO[g])) : "memory");
     }
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) {
@@ -279,6 +416,7 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
   const int wg = (warp >> 2) - 1, t = threadIdx.x & 127;
   const int r0 = (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
   const bool stamper = wg == 0 && t == 0;
+  const uint32_t stg = smem_u32(smem) + STAGES * STAGE_BYTES + wg * TC_STG_BYTES;
   constexpr long long SLOT_FLOATS = (long long)TC_BLOCK_M * BLOCK_N;
   // a stage is free again for the producers that write it: this CTA's, and the peer's (its half
   // of W)
@@ -356,6 +494,19 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
         for (int pi = 0; pi < seg.n_peers; ++pi) sc.sk_flags[(peer_cta0 + pi * CLUSTER) * 8 + wg] = 0;
     }
     if (stamper) TC_STAMP(5);
+    if (e.staged) {
+      // through shared memory and TMA stores, left draining under the next segment's main loop
+      auto first_wait = [] { bulk_wait_read0(); };
+      auto written = [&] { if (stamper) TC_STAMP(6); };
+      if (p.out_mode == OUT_S2D_BF16)
+        staged_epilogue<BLOCK_N, TC_STG_COLS>(d, stg, n0, p.N, p.bias, p.relu, StgS2D(&args.tmO[g], p.N, m0),
+                                              first_wait, written);
+      else
+        staged_epilogue<BLOCK_N, TC_STG_COLS>(d, stg, n0, p.N, p.bias, p.relu, StgRowMajor{&args.tmO[g], m0},
+                                              first_wait, written);
+      if (stamper) TC_STAMP(7);
+      continue;
+    }
     const int pN = p.N, pM = p.M, prelu = p.relu, pmode = p.out_mode;
     const float* pbias = p.bias;
     void* pout = p.out;
@@ -402,6 +553,7 @@ k_gemm_tc_persistent(const __grid_constant__ TcArgs args, const TcSched sc) {
     }
     if (stamper) { TC_STAMP(6); TC_STAMP(7); }
   }
+  if (e.staged && t == 0) bulk_wait_read0();   // the staging buffer is read before the CTA leaves
   // no CTA leaves while its peer may still multicast into it or arrive on its barriers
   if constexpr (CLUSTER > 1) cluster_sync();
 }
@@ -486,10 +638,7 @@ __device__ __forceinline__ void heads_unit(const HeadsArgs& args, uint32_t smem,
                                            uint64_t* full_bar, uint64_t* empty_bar, uint32_t peer_empty,
                                            int u, int crank, int& kc, int& pending) {
   constexpr int STAGE_BYTES = TC_A_BYTES + 256 * TC_BLOCK_K * 2;
-  constexpr int H = BN < HC ? BN : HC;        // columns per staging pass
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int wg = (warp >> 2) - 1, t = threadIdx.x & 127;
-  const int r0 = (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
+  const int wg = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127;
   int q, mp, nt;
   hd_decode(args, u, q, mp, nt);
   const int kbn = args.kb[q];
@@ -526,42 +675,13 @@ __device__ __forceinline__ void heads_unit(const HeadsArgs& args, uint32_t smem,
   const float* pbias = args.bias[q];
   const int pN = args.N[q], prelu = args.relu[q];
   const int m0 = (2 * mp + crank) * TC_BLOCK_M + wg * 64, n0 = nt * BN;
-  // thread's element (row r, column c) of a 64 x 64 box sits at r x 128 + ((c / 8) ^ (r % 8)) x 16
-  // + (c % 8) x 2 (SW128; r % 8 = lane / 4 for both of its rows): the 32 lanes of a store hit
-  // 32 distinct banks
-  const uint32_t rowa = stg + r0 * 128 + cq * 2, sw = (uint32_t)(lane >> 2);
-  // one loop over the fragment's column groups j (fully unrolled, so d[] stays in registers); a
-  // staging pass starts every H / 8 of them
-#pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int jj = j % (H / 8);
-    if (jj == 0) {
-      if (t == 0) {
-        if (j == 0 && pending >= 0) { hd_publish(args, pending); pending = -1; }
-        else bulk_wait_read0();        // the staging buffer's previous stores have read it
-      }
-      wg_bar(1 + wg);
-    }
-    const int n = n0 + 8 * j + cq;
-    const bool in = n < pN;
-    const float b0 = (pbias && in) ? __ldg(pbias + n) : 0.f, b1 = (pbias && in) ? __ldg(pbias + n + 1) : 0.f;
-    const uint32_t at = rowa + (jj >> 3) * 8192 + ((((uint32_t)jj & 7) ^ sw) << 4);
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const float x0 = d[4 * j + 2 * i] + b0, x1 = d[4 * j + 2 * i + 1] + b1;
-      sts_b32(at + i * 8 * 128, prelu ? pack_bf16x2_relu(x0, x1) : pack_bf16x2(x0, x1));
-    }
-    if (jj == H / 8 - 1) {
-      fence_proxy_async_smem();
-      wg_bar(1 + wg);
-      if (t == 0) {
-        const int c0 = n0 + (j / (H / 8)) * H;
-#pragma unroll
-        for (int b = 0; b < H / 64; ++b) tma_store_2d(&args.tmO[q], stg + b * 8192, c0 + 64 * b, m0);
-        bulk_commit();
-      }
-    }
-  }
+  // before the first pass: publish the tile whose signal was held back, or wait for the staging
+  // buffer's previous stores to have read it
+  auto first_wait = [&] {
+    if (pending >= 0) { hd_publish(args, pending); pending = -1; }
+    else bulk_wait_read0();
+  };
+  staged_epilogue<BN, HC>(d, stg, n0, pN, pbias, prelu, StgRowMajor{&args.tmO[q], m0}, first_wait, [] {});
 }
 
 template <int STAGES, int HC>
@@ -741,9 +861,11 @@ static int encode(CUtensorMap* tm, const void* base, int rank, const cuuint64_t*
   return r == CUDA_SUCCESS ? MF_OK : MF_E_BADARG;
 }
 
+// the stage ring, the two consumer warpgroups' staging buffers and 1 KB for the alignment:
+// 4 x 48 KB or 6 x 32 KB, + 32 KB + 1 KB = 225 KB of the 227 KB a block may use
 template <int BLOCK_N, int STAGES>
 static constexpr int persistent_smem() {
-  return STAGES * (TC_A_BYTES + BLOCK_N * TC_BLOCK_K * 2) + 1024;
+  return STAGES * (TC_A_BYTES + BLOCK_N * TC_BLOCK_K * 2) + 2 * TC_STG_BYTES + 1024;
 }
 
 template <int BLOCK_N, int STAGES>
@@ -847,6 +969,34 @@ static int make_maps(const GemmParams& p, int w_rows, CUtensorMap* tmA, CUtensor
   return encode(tmW, p.W, 2, dims, str, box);
 }
 
+// Whether a bf16 output can leave through the staged epilogue (staged_epilogue): row-major with
+// a 16-byte aligned first column and pitch, or s2d at Do = 16 whose slots are whole 64-channel
+// boxes.  fp32 outputs, ragged N and anything a TMA store cannot address take the register path.
+static bool staged_ok(const GemmParams& p) {
+  if (p.N % 32 != 0) return false;
+  if (p.out_mode == OUT_BF16)
+    return ((uintptr_t)p.out + 2 * (uintptr_t)p.col_off) % 16 == 0 && p.ldo % 8 == 0 && p.ldo >= p.N;
+  if (p.out_mode == OUT_S2D_BF16)
+    return p.Do == 16 && p.N % 64 == 0 && p.M % 4096 == 0 && (uintptr_t)p.out % 16 == 0;
+  return false;
+}
+
+// Output map of the staged epilogue: row-major {N, M} at out + col_off in 64 x 64 boxes, or the
+// s2d layout [B][9][9][9][8 N] of the next convolution's input in {64, 8, 2, 1, 1} boxes (StgS2D)
+static int make_out_map(const GemmParams& p, CUtensorMap* tm) {
+  if (p.out_mode == OUT_S2D_BF16) {
+    const cuuint64_t J = 9, C = 8 * (cuuint64_t)p.N;
+    const cuuint64_t dims[5] = {C, J, J, J, (cuuint64_t)(p.M / 4096)};
+    const cuuint64_t str[4] = {C * 2, J * C * 2, J * J * C * 2, J * J * J * C * 2};
+    const cuuint32_t box[5] = {64, 8, 2, 1, 1};
+    return encode(tm, p.out, 5, dims, str, box);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)p.N, (cuuint64_t)p.M};
+  const cuuint64_t str[1] = {(cuuint64_t)p.ldo * 2};
+  const cuuint32_t box[2] = {64, 64};
+  return encode(tm, reinterpret_cast<const bf16*>(p.out) + p.col_off, 2, dims, str, box);
+}
+
 }  // namespace mf
 
 using namespace mf;
@@ -927,6 +1077,14 @@ extern "C" int mf_gemm_bf16_tc_ex(const GemmParams* hp, int n_groups, void* work
     if (!workspace || workspace_bytes < (size_t)splitk * p0.M * p0.N * 4) return MF_E_WORKSPACE;
     args.e.ws = (float*)workspace;
   }
+  // bf16 outputs leave through shared memory and TMA stores when every group's output allows it
+  bool staged = splitk == 1;
+  for (int g = 0; g < n_groups; ++g) staged = staged && staged_ok(hp[g]);
+  for (int g = 0; staged && g < n_groups; ++g) {
+    int rc = make_out_map(hp[g], &args.tmO[g]);
+    if (rc) return rc;
+  }
+  args.e.staged = staged ? 1 : 0;
   const int m_units = m_tiles / cluster;
   TcSched sc{m_units, n_tiles, n_groups, splitk, m_units * n_tiles * n_groups * splitk,
              stamps, streamk ? 1 : 0, sync, (float*)workspace};
@@ -1023,10 +1181,7 @@ extern "C" int mf_cnn_heads_tc(const GemmParams* layers, int n_layers, int32_t* 
     int dummy = 0;
     int rc = make_maps(p, bn[q] / 2, &a.tmA[q], &a.tmW[q], &dummy);
     if (rc) return rc;
-    const cuuint64_t dims[2] = {(cuuint64_t)p.N, (cuuint64_t)p.M};
-    const cuuint64_t str[1] = {(cuuint64_t)p.ldo * 2};
-    const cuuint32_t box[2] = {64, 64};
-    rc = encode(&a.tmO[q], reinterpret_cast<const bf16*>(p.out) + p.col_off, 2, dims, str, box);
+    rc = make_out_map(p, &a.tmO[q]);
     if (rc) return rc;
   }
   a.unit_begin[HD_GEMMS] = units;
