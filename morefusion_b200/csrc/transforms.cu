@@ -206,7 +206,9 @@ extern "C" int mf_transform_points_bwd(const float* gout, const float* points, i
   cudaStream_t stream = (cudaStream_t)stream_;
   if (P < 0 || M < 0) return MF_E_BADARG;
   if (P == 0 || M == 0) {
+    // empty sums: both gradients are zero, not whatever the caller's buffers held
     if (gT && M > 0) MF_CUDA_TRY(cudaMemsetAsync(gT, 0, (size_t)M * 64, stream));
+    if (gpoints && P > 0) MF_CUDA_TRY(cudaMemsetAsync(gpoints, 0, (size_t)P * 12, stream));
     return MF_OK;
   }
   if (!gout || !points || !T) return MF_E_BADARG;

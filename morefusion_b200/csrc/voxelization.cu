@@ -370,8 +370,13 @@ __global__ void k_avg_bwd(const float* __restrict__ gmatrix, const int* __restri
 }
 
 // ---------------------------------------------------------------- max voxelization
+// order-preserving bits of a float.  -0 is folded onto +0 (-0 + 0 = +0 in round-to-nearest) so
+// that the two compare equal, as `intensity > max_intensity` has them, and the lower point id
+// wins.  The reference's result with a NaN intensity depends on arrival order (`>` is false both
+// ways, so the first arrival keeps the voxel); here a NaN of either sign ranks above every number.
 __device__ __forceinline__ unsigned int f2ord(float f) {
-  unsigned int u = __float_as_uint(f);
+  if (f != f) return 0xffffffffu;
+  unsigned int u = __float_as_uint(__fadd_rn(f, 0.f));
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
