@@ -183,9 +183,11 @@ def backward_pcd(model, values, class_id, g_rot, g_trans, g_conf, needs_values=F
                                       ptr(tb["dpooled"]), s()), "obj_bias_bwd")
         model._gemm(L, dz1, tw["head1/Wt"], None, tb["dfeat"], NP, FEAT12, 1920, lda=1920, relu=0,
                     out_mode=OUT_F32, ldo=FEAT12)
+        # added like every other gradient: under a Trainer the destinations are .grad views that a
+        # second backward before zero_grad() accumulates into (gw1 / gb1 are zeroed above)
         for i, h in enumerate(HEADS):
-            G[f"conv1_{h}.weight"].view(640, 1408).copy_(tb["gw1"][i * 640:(i + 1) * 640])
-            G[f"conv1_{h}.bias"].copy_(tb["gb1"][i * 640:(i + 1) * 640])
+            G[f"conv1_{h}.weight"].view(640, 1408).add_(tb["gw1"][i * 640:(i + 1) * 640])
+            G[f"conv1_{h}.bias"].add_(tb["gb1"][i * 640:(i + 1) * 640])
         if on_bucket:
             on_bucket("heads")
         # ---- the mean over the points, conv4, conv3
