@@ -721,7 +721,28 @@ int mf_psp_tail_sampled(const float* up2_nhwc, const int64_t* pix, int B, int P,
  *     an instance whose centre_set [n_instances] int32 is 0 and that pushed at least one point
  *     gets centre_set = 1 and centres [n_instances,3] f32 = the mean of its listed world points of
  *     this scan, range or not, except the lowest pixel index, summed exactly in fixed point
- *     (2^-32 m).  Three launches, stream-ordered, no host sync.
+ *     (2^-32 m).  Boxes: boxes [n_instances,6] u32 hold each instance's (min xyz, max xyz) in an
+ *     order-preserving encoding of the floats (negative: bits inverted; otherwise the sign bit
+ *     set; a zero is +0); OctoMap's default box (0,0,0)-(0,0,0) at allocation.  tree_state
+ *     [n_instances] int32: 1 where the instance has a tree in the server's sense, 0 where not yet;
+ *     the scan creates the tree of every instance whose id its labels hold on any pixel (odd rows
+ *     and columns and NaN points included, unique(label_ins), :290-319) and sets the flag.  Each
+ *     instance other than the background that pushed a point widens its box by those points (the
+ *     first excluded) as insertScan's setBBXMin/Max do (:404-437); an instance whose tree this
+ *     scan created takes the min / max of them instead, (+FLT_MAX, -FLT_MAX) when there are none,
+ *     and keeps the default box when it has no listed point.  Five launches, stream-ordered, no
+ *     host sync.
+ * mf_map_render: the server's render (OctomapServer::render, :193-281) of the map into the
+ *     camera of an organised camera-frame cloud points [height*width,3] f32 (sensor_to_world as
+ *     above; fx, fy, cx, cy the intrinsics rounded to float).  walk / walk_ids [n_walk] int32:
+ *     dense index / instance id of each rendered instance in ascending id order (the background
+ *     left out); boxes as above.  Every even pixel casts castRay(origin, point - origin,
+ *     ignoreUnknownCells, 1.1 |point - origin|) into each instance whose box holds its world
+ *     point, or, with no depth, to the z = 1 point of its ray with no box test; the nearest hit
+ *     (the lower id on a tie) writes its distance to depth [height,width] f32 at the pixel and
+ *     its id to label [height,width] int32 on rows v-1..v, columns u-1..u; the rest is
+ *     `uncertain` / NaN.  zbuf: workspace of ((height+1)/2)*((width+1)/2) u64.  Two launches
+ *     and a memset, stream-ordered, no host sync.
  * mf_map_server_grid_params: publishGrids' pitch [T] f64 (the instance's resolution) and origin
  *     [T,3] f64 of T targets (dense indices, device) from their world centres: the centre moved
  *     by world_to_sensor (HOST [12] f32) in float, minus (off_x, off_y, off_z) * pitch in double
@@ -763,7 +784,12 @@ int mf_map_integrate_server(const float* points, const int32_t* labels, int heig
                             uint32_t scan, float hit, float miss, float lo_min, float lo_max,
                             void* centre_sums, uint32_t* centre_first, float* centres,
                             int32_t* centre_set, void* cells, void* cnt, int64_t capacity,
-                            int32_t* counters, void* stream);
+                            int32_t* counters, int32_t* tree_state, uint32_t* boxes, void* stream);
+int mf_map_render(const float* points, int height, int width, const float* sensor_to_world,
+                  float fx, float fy, float cx, float cy, const int32_t* walk,
+                  const int32_t* walk_ids, int n_walk, const double* inst_resolution,
+                  const uint32_t* boxes, int uncertain, void* zbuf, int32_t* label, float* depth,
+                  void* cells, void* cnt, int64_t capacity, int32_t* counters, void* stream);
 int mf_map_server_grid_params(const int32_t* target_index, int T, const double* inst_resolution,
                               const float* centres, const float* world_to_sensor, double off_x,
                               double off_y, double off_z, double* pitch, double* origin,

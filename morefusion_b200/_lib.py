@@ -115,7 +115,9 @@ SIGNATURES = {
                                              c_p, c_i, c_p, c_p, c_i64, c_p, c_p, c_p, c_p]),
     "mf_map_integrate_server": (c_i, [c_p, c_p, c_i, c_i, c_p, c_d, c_p, c_i, c_i, c_p, c_i, c_i, c_d,
                                        c_i, ctypes.c_uint32, c_f, c_f, c_f, c_f, c_p, c_p, c_p, c_p,
-                                       c_p, c_p, c_i64, c_p, c_p]),
+                                       c_p, c_p, c_i64, c_p, c_p, c_p, c_p]),
+    "mf_map_render": (c_i, [c_p, c_i, c_i, c_p, c_f, c_f, c_f, c_f, c_p, c_p, c_i, c_p, c_p, c_i,
+                            c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_p]),
     "mf_map_server_grid_params": (c_i, [c_p, c_i, c_p, c_p, c_p, c_d, c_d, c_d, c_p, c_p, c_p]),
     "mf_objmap_state_bytes": (c_sz, [c_i]),
     "mf_objmap_append": (c_i, [c_p, c_i, c_p, c_i, c_p, c_p, c_p, c_p, c_i, c_p]),

@@ -26,6 +26,9 @@ import torch
 from .. import _lib
 
 _TREE_MAX_VAL = 32768
+# an instance box as stored on the device ([6] of box_enc, csrc/mapping.cu): OctoMap's default box
+# (0,0,0)-(0,0,0), the sign bit set on +0's bits
+_BOX_DEFAULT = -(1 << 31)
 
 
 def _logodds(p):
@@ -81,12 +84,17 @@ class MultiInstanceOctreeMapping:
         self._pending = None                     # event of the last asynchronous counter read-back
         self._res_factor = None                  # cached device array of 1 / pitch
         self._lut = None                         # cached (lut, lut_lo, resolutions) device arrays
+        self._res = None                         # cached device array of every instance's resolution
         self._query_cache = None                 # cached (key, targets, pitches, origins) device arrays
         self._walk = None                        # cached (background id, walk order, its dense index)
+        self._render_walk = None                 # cached (background id, walk [2, n] device array)
         # integrate_scan's per-instance world centres (by dense index), their "set" flags, the
-        # scan's centre accumulators, and a host mirror of the flags (True = known to be set)
+        # scan's centre accumulators, and a host mirror of the flags (True = known to be set);
+        # the instance boxes that render reads, and whether the server would have created the
+        # instance's tree yet (1) or not (0: listed to integrate_scan, never in its labels)
         self._centres = self._centre_set = self._centre_sums = self._centre_first = None
         self._centre_known = None
+        self._boxes = self._tree_state = None
 
     # ------------------------------------------------------------------ table management
     def _alloc_table(self, cap):
@@ -166,7 +174,9 @@ class MultiInstanceOctreeMapping:
         self._pitch.append(float(pitch))
         self._res_factor = None
         self._lut = None
+        self._res = None
         self._walk = None
+        self._render_walk = None
 
     def integrate(self, instance_id, mask, pcd, origin=(0, 0, 0)):
         """octree.insertPointCloud(pcd[mask & nonnan], origin) (:21-27).  mask [H,W] bool, pcd
@@ -309,7 +319,7 @@ class MultiInstanceOctreeMapping:
     def integrate_scan(self, label, pcd, sensor_to_world, class_ids, *, max_range=-1.0,
                        background_id=-1, uncertain_id=-2, background_pitch=0.01):
         """One frame of a moving camera into the map in the world frame, as the ROS occupancy
-        server's ``insertScan`` does it (OctomapServer.cpp:283-448); three launches, no host sync.
+        server's ``insertScan`` does it (OctomapServer.cpp:283-448); five launches, no host sync.
 
         label [H,W] integer image, pcd [H,W,3] organised camera-frame cloud (NaN = no depth),
         sensor_to_world [4,4] host array, class_ids {instance_id: class_id}.
@@ -336,7 +346,12 @@ class MultiInstanceOctreeMapping:
         too, except the one of lowest pixel index (the server does not push an instance's first
         point, :345-349).  The sum is exact in a fixed point of 2^-32 m, so it does not depend
         on thread order.  An instance with no pushed point has no centre yet (the server would
-        read an uninitialised centroid)."""
+        read an uninitialised centroid).
+
+        Each instance other than the background keeps a box (``boxes``, read by ``render``),
+        widened by the points it pushed (insertScan's setBBXMin/Max, :404-437); in the first scan
+        whose labels hold its id on any pixel (where the server creates its tree) the box is set
+        to those points alone."""
         from .singleview_3d.models.model import YCB_VOXEL_PITCH_32
         dev = self.device
         T = _matrix4f(sensor_to_world)
@@ -359,18 +374,20 @@ class MultiInstanceOctreeMapping:
                 raise IndexError(f"class_id {c} out of range")
         if not background_pitch > 0:
             raise ValueError("background_pitch must be positive")
+        first_new = len(self._pitch)       # created below: no tree until the labels hold them
         for i, c in classes.items():
             if i not in self._ids:
                 self.initialize(i, pitch=YCB_VOXEL_PITCH_32[c])
         if background_id not in self._ids:
             self.initialize(background_id, pitch=background_pitch)
+        self._ensure_centres()
+        self._tree_state[first_new:len(self._pitch)] = 0
         H, W = int(pts.shape[0]), int(pts.shape[1])
         lab = lab.to(torch.int32).contiguous()
         self._check(wait=False)
         if H * W == 0:
             return
         lut, lo, res = self._label_lut()
-        self._ensure_centres()
         bg = self._ids[background_id]
         self._scan += 1
         with self._dev_ctx():
@@ -380,7 +397,9 @@ class MultiInstanceOctreeMapping:
                 self._pitch[bg], int(uncertain_id), self._scan, float(self._hit), float(self._miss),
                 float(self._lo_min), float(self._lo_max), _lib.ptr(self._centre_sums),
                 _lib.ptr(self._centre_first), _lib.ptr(self._centres), _lib.ptr(self._centre_set),
-                *self._table_args(), _lib.stream()), "map_integrate_server")
+                *self._table_args(), _lib.ptr(self._tree_state), _lib.ptr(self._boxes),
+                _lib.stream()),
+                "map_integrate_server")
             self._read_back()
 
     def server_grid_params(self, target_ids, sensor_to_world, dimensions=(32, 32, 32)):
@@ -448,14 +467,19 @@ class MultiInstanceOctreeMapping:
         centres = torch.zeros((new, 3), dtype=torch.float32, device=dev)
         cset = torch.zeros(new, dtype=torch.int32, device=dev)
         known = np.zeros(new, bool)
+        boxes = torch.full((new, 6), _BOX_DEFAULT, dtype=torch.int32, device=dev)
+        trees = torch.ones(new, dtype=torch.int32, device=dev)
         if cap:
             sums[:cap] = self._centre_sums
             first[:cap] = self._centre_first
             centres[:cap] = self._centres
             cset[:cap] = self._centre_set
             known[:cap] = self._centre_known
+            boxes[:cap] = self._boxes
+            trees[:cap] = self._tree_state
         self._centre_sums, self._centre_first = sums, first
         self._centres, self._centre_set, self._centre_known = centres, cset, known
+        self._boxes, self._tree_state = boxes, trees
 
     def centres(self):
         """{instance_id: world centre float32 [3]} of the instances that have one (host read;
@@ -464,6 +488,76 @@ class MultiInstanceOctreeMapping:
         c = self._centres.cpu().numpy()
         s = self._centre_set.cpu().numpy()
         return {i: c[q].copy() for i, q in self._ids.items() if s[q]}
+
+    def boxes(self, background_id=-1):
+        """{instance_id: float32 [2, 3] (min, max)} of every instance but the background: the box
+        ``integrate_scan`` keeps and ``render`` tests points against.  An instance that no scan
+        has boxed has OctoMap's default box, all zeros.  (Host read; for tests and tools.)"""
+        self._ensure_centres()
+        if not self._ids:
+            return {}
+        e = self._boxes[:len(self._pitch)].cpu().numpy().view(np.uint32)
+        bits = np.where(e & 0x80000000, e & 0x7FFFFFFF, ~e).astype(np.uint32)
+        b = bits.view(np.float32).reshape(-1, 2, 3)
+        return {i: b[q].copy() for i, q in self._ids.items() if i != background_id}
+
+    def render(self, pcd, sensor_to_world, K, *, background_id=-1, uncertain_id=-2):
+        """The map's own label image of the current view, as the ROS occupancy server's
+        ``render`` draws it (OctomapServer.cpp:193-281).  Returns CUDA tensors label [H, W]
+        int32 and depth [H, W] float32; two launches, no host sync.
+
+        pcd [H, W, 3] organised camera-frame cloud (NaN = no depth) and sensor_to_world [4, 4]
+        (host) as ``integrate_scan`` takes them, K [3, 3] host intrinsics.  For every pixel of
+        even row and column and every instance but ``background_id``: a pixel with depth is moved
+        to the world as in ``integrate_scan`` and is skipped unless it lies in the instance's box
+        (``boxes``); a pixel without depth targets the z = 1 point of its ray, (u - cx) / fx,
+        (v - cy) / fy in float, with no box test.  OctoMap's castRay from the sensor origin
+        towards the target, unknown cells ignored, up to 1.1 times the target's distance, finds
+        the first occupied cell of the instance (log-odds >= 0) in its own key space.  Of the
+        instances hit, the nearest cell centre wins the pixel -- on an exact tie the lower
+        instance id, as the server run on one thread --: its float distance is depth[v, u] and its
+        id fills label[v-1:v+1, u-1:u+1] (clipped at the image edge).  Every other label pixel is
+        ``uncertain_id``, every other depth pixel NaN."""
+        dev = self.device
+        T = _matrix4f(sensor_to_world)
+        K = np.asarray(K, np.float64).reshape(3, 3)
+        if not np.isfinite(K).all():
+            raise ValueError("K must be finite")
+        fx, fy, cx, cy = (float(np.float32(k)) for k in (K[0, 0], K[1, 1], K[0, 2], K[1, 2]))
+        pts = torch.as_tensor(pcd).to(device=dev, dtype=torch.float32).contiguous()
+        if pts.dim() != 3 or pts.shape[2] != 3:
+            raise ValueError("pcd must be [H,W,3]")
+        _lib.require_cuda(pts)
+        H, W = int(pts.shape[0]), int(pts.shape[1])
+        label = torch.empty((H, W), dtype=torch.int32, device=dev)
+        depth = torch.empty((H, W), dtype=torch.float32, device=dev)
+        self._check(wait=False)
+        if H * W == 0:
+            return label, depth
+        if self._render_walk is None or self._render_walk[0] != background_id:
+            ids = sorted(i for i in self._ids if i != background_id)       # the server's std::map order
+            walk = np.asarray([[self._ids[i] for i in ids], ids], np.int64).reshape(2, -1)
+            if walk.size and not (np.abs(walk[1]) < 1 << 31).all():
+                raise ValueError("instance ids must fit in int32 to be rendered")
+            self._render_walk = (background_id, torch.as_tensor(walk.astype(np.int32)).to(dev))
+        walk = self._render_walk[1]
+        n_walk = walk.shape[1]
+        self._ensure_centres()
+        res = self._resolutions() if n_walk else None
+        zbuf = torch.empty(((H + 1) // 2) * ((W + 1) // 2), dtype=torch.int64, device=dev)
+        with self._dev_ctx():
+            _lib.check(_lib.lib().mf_map_render(
+                _lib.ptr(pts), H, W, _host_xform(T), fx, fy, cx, cy, _lib.ptr(walk[0]),
+                _lib.ptr(walk[1]), n_walk, _lib.ptr(res), _lib.ptr(self._boxes), int(uncertain_id),
+                _lib.ptr(zbuf), _lib.ptr(label), _lib.ptr(depth), *self._table_args(),
+                _lib.stream()), "map_render")
+        return label, depth
+
+    def _resolutions(self):
+        """Cached float64 device array of every instance's resolution, by dense index."""
+        if self._res is None:
+            self._res = torch.as_tensor(np.asarray(self._pitch, dtype=np.float64)).to(self.device)
+        return self._res
 
     def _label_lut(self):
         """Cached (lut, lut_lo, resolutions) device arrays: label - lut_lo -> dense index."""
@@ -476,8 +570,7 @@ class MultiInstanceOctreeMapping:
             for i, idx in self._ids.items():
                 lut[int(i) - lo] = idx
             dev = self.device
-            self._lut = (torch.as_tensor(lut).to(dev), lo,
-                         torch.as_tensor(np.asarray(self._pitch, dtype=np.float64)).to(dev))
+            self._lut = (torch.as_tensor(lut).to(dev), lo, self._resolutions())
         return self._lut
 
     def _query_args(self, target_ids, dimensions, pitches, origins):

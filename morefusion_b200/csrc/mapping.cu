@@ -29,7 +29,10 @@
 //                     pair, with the occupancy server's rules (OctomapServer.cpp:510-618);
 //                     k_map_query_node_grids_world the same with camera-frame origins.
 //   k_map_server_hits / k_map_scan_free<ServerScanParams> / k_map_server_centres  the server's
-//                     scan of a moving camera's frame in the world frame (insertScan, :283-448).
+//                     scan of a moving camera's frame in the world frame (insertScan, :283-448);
+//                     k_map_server_boxes the instance boxes that scan keeps (:404-437).
+//   k_map_render_rays / k_map_render_write  the server's render of the map into the camera
+//                     (:193-281): castRay per (even pixel, instance), a per-pixel z-buffer.
 // A cell is updated by exactly one thread per scan, so results do not depend on thread order:
 // bit-identical to the serial oracle.  -fmad=false: the double expressions must not contract.
 #include <math.h>
@@ -38,6 +41,7 @@
 // tests/emu/mapping_emu.cpp runs the kernels of this file serially on the host (one-lane "warps")
 // against oracle/octomap.py in the CPU test suite; it supplies the CUDA spellings used below.
 #include "mapping_emu_stubs.h"
+#include "mapping_render_emu_stubs.h"
 #else
 #include "common.cuh"
 #endif
@@ -211,14 +215,19 @@ __device__ __forceinline__ bool server_point(const ServerScanParams& p, int i, f
   return *q >= 0;
 }
 
-// (point - sensorOrigin): the float difference and its point3d::norm(), sqrt of the float norm_sq
-__device__ __forceinline__ double server_ray(const ServerScanParams& p, const float w[3], float d[3]) {
-  d[0] = __fsub_rn(w[0], p.ox);
-  d[1] = __fsub_rn(w[1], p.oy);
-  d[2] = __fsub_rn(w[2], p.oz);
+// (point - origin): the float difference and its point3d::norm(), sqrt of the float norm_sq
+__device__ __forceinline__ double point_diff_norm(const float w[3], float ox, float oy, float oz,
+                                                  float d[3]) {
+  d[0] = __fsub_rn(w[0], ox);
+  d[1] = __fsub_rn(w[1], oy);
+  d[2] = __fsub_rn(w[2], oz);
   const float nsq = __fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])),
                               __fmul_rn(d[2], d[2]));
   return sqrt((double)nsq);
+}
+
+__device__ __forceinline__ double server_ray(const ServerScanParams& p, const float w[3], float d[3]) {
+  return point_diff_norm(w, p.ox, p.oy, p.oz, d);
 }
 
 // pcl::compute3DCentroid's sum in a fixed point of 2^-32 m: integer sums do not depend on the
@@ -363,6 +372,80 @@ k_map_server_centres(ServerScanParams p, int n_inst, float* __restrict__ centres
   }
   acc[0] = acc[1] = acc[2] = acc[3] = 0ull;
   p.cfirst[q] = 0u;
+}
+
+// An instance box as [6] u32: box_enc of (min x, y, z, max x, y, z).  box_enc orders like the
+// floats it encodes (non-NaN), so atomicMin / atomicMax on it give the exact float min / max in
+// any order of the atomics.  A zero is encoded as +0: the server's sign of a zero bound depends
+// on its OpenMP order, and inBBX does not see it.
+__device__ __forceinline__ unsigned box_enc(float f) {
+  const unsigned b = __float_as_uint(f == 0.f ? 0.f : f);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+__device__ __forceinline__ float box_dec(unsigned e) {
+  return __uint_as_float((e & 0x80000000u) ? (e & 0x7fffffffu) : ~e);
+}
+
+// The server creates an instance's tree in the first scan whose label image holds its id on any
+// pixel -- odd rows and columns and NaN points included -- (unique(label_ins), :290-319), and in
+// that scan its box is set to, not widened by, the min / max of the points it pushes (:425-432).
+// tree [n_inst] int32: 0 = no tree yet, 1 = a tree, 2 = created by this scan (until
+// k_map_server_boxes).  One thread per pixel, before k_map_server_boxes: the thread that creates
+// a tree opens its box at pcl::getMinMax3D of no point, (+FLT_MAX, -FLT_MAX).
+__global__ void __launch_bounds__(256)
+k_map_server_trees(ServerScanParams p, int* __restrict__ tree, unsigned* __restrict__ box) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p.n) return;
+  const int l = p.labels[i] - p.lut_lo;
+  const int q = (l >= 0 && l < p.lut_n) ? p.lut[l] : -1;
+  if (q < 0 || q == p.bg || tree[q] != 0 || atomicCAS(tree + q, 0, 2) != 0) return;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    box[6 * q + a] = box_enc(3.402823466e38f);
+    box[6 * q + 3 + a] = box_enc(-3.402823466e38f);
+  }
+}
+
+// The boxes (:404-437), after k_map_server_hits (which leaves each instance's point count in
+// csum and its first pixel in cfirst) and before k_map_server_centres (which resets both).  Every
+// point the server pushes -- a listed point of an instance other than the background, range or
+// not, except the instance's first of the scan -- widens its instance's box.  An instance with
+// exactly one point pushes none and gets no widening: one whose tree this scan created keeps
+// the empty box, an older one its box.  An instance whose tree this scan created with no listed
+// point (its id only on odd rows / columns or NaN points) is not boxed by the server and keeps
+// OctoMap's default box (0,0,0)-(0,0,0); thread q (< n_inst) restores it and marks the tree as
+// existing.
+__global__ void __launch_bounds__(256)
+k_map_server_boxes(ServerScanParams p, int n_inst, int* __restrict__ tree,
+                   unsigned* __restrict__ box) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_inst && tree[i] == 2) {
+    if (p.csum[4 * i + 3] == 0ull) {
+#pragma unroll
+      for (int a = 0; a < 6; ++a) box[6 * i + a] = box_enc(0.f);
+    }
+    tree[i] = 1;
+  }
+  float w[3];
+  int q;
+  const bool push = server_point(p, i, w, &q) && q >= 0 && q != p.bg &&
+                    (unsigned)i != ~p.cfirst[q];
+  // the pushing lanes of a warp (neighbouring pixels of one row) mostly share an instance: each
+  // instance's lanes reduce first, and one of them issues the atomics
+  const unsigned act = __ballot_sync(0xffffffffu, push);
+  if (!push) return;
+  const unsigned peers = __match_any_sync(act, q);
+  const bool lead = (__ffs(peers) - 1) == (int)(threadIdx.x & 31);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const unsigned lo = __reduce_min_sync(peers, box_enc(w[a]));
+    const unsigned hi = __reduce_max_sync(peers, box_enc(w[a]));
+    if (lead) {
+      atomicMin(box + 6 * q + a, lo);
+      atomicMax(box + 6 * q + 3 + a, hi);
+    }
+  }
 }
 
 // The key ray of computeRayKeys (oracle/octomap.py::OcTree.computeRayKeys has the line-by-line
@@ -649,6 +732,145 @@ k_map_server_grid_params(const int* __restrict__ target_index, int T,
   origin[3 * tg + 2] = (double)c[2] - off_z * pt;
 }
 
+// OccupancyOcTreeBase::castRay(origin, dir, end, ignoreUnknownCells = true, max_range) in
+// instance q's key space; oracle/octomap_server_render.py::cast_ray restates it line by line.
+// True with `end` = the centre of the first occupied cell (isNodeOccupied: log-odds >= 0) on the
+// ray, the origin's own cell included; unknown and free cells are passed.  False when the origin
+// is outside the key range, the direction is zero, a key would leave the range, or a cell centre
+// lies beyond max_range (> 0; otherwise no limit).  Every DDA step is taken: tMax accumulates
+// its rounding in sequence, as the library's does.
+__device__ __forceinline__ bool cast_ray(const MapTable& t, int q, double res, const float o[3],
+                                         const float dir[3], double max_range, float end[3]) {
+  const double rf = 1.0 / res;
+  int cur[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    cur[a] = coord_to_key((double)o[a], rf);
+    if (cur[a] < 0) return false;
+  }
+  MapCell c;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) end[a] = (float)(((double)(cur[a] - TREE_MAX_VAL) + 0.5) * res);
+  if (map_find(t, pack_key(q, cur[0], cur[1], cur[2]), &c) >= 0 && c.lo >= 0.f) return true;
+  // direction.normalized(): divided by the float of point3d::norm() when that is > 0
+  float dn[3];
+  const double len = point_diff_norm(dir, 0.f, 0.f, 0.f, dn);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) dn[a] = len > 0.0 ? __fdiv_rn(dir[a], (float)len) : dir[a];
+  int step[3];
+  double tmax[3], tdelta[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    step[a] = dn[a] > 0.f ? 1 : (dn[a] < 0.f ? -1 : 0);
+    if (step[a] != 0) {
+      // castRay keeps the half step in double (computeRayKeys rounds it to float)
+      double border = ((double)(cur[a] - TREE_MAX_VAL) + 0.5) * res;
+      border += (double)step[a] * res * 0.5;
+      tmax[a] = (border - (double)o[a]) / (double)dn[a];
+      tdelta[a] = res / fabs((double)dn[a]);
+    } else {
+      tmax[a] = 1.7976931348623157e308;
+      tdelta[a] = 1.7976931348623157e308;
+    }
+  }
+  if (step[0] == 0 && step[1] == 0 && step[2] == 0) return false;
+  const bool range_set = max_range > 0.0;
+  const double range_sq = max_range * max_range;
+  for (;;) {
+    const int dim = tmax[0] < tmax[1] ? (tmax[0] < tmax[2] ? 0 : 2) : (tmax[1] < tmax[2] ? 1 : 2);
+    bool out = false;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      if (a != dim) continue;
+      out = (step[a] < 0 && cur[a] == 0) || (step[a] > 0 && cur[a] == 2 * TREE_MAX_VAL - 1);
+      cur[a] += step[a];
+      tmax[a] += tdelta[a];
+    }
+    if (out) return false;
+    double dsq = 0.0;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      end[a] = (float)(((double)(cur[a] - TREE_MAX_VAL) + 0.5) * res);
+      const float e = __fsub_rn(end[a], o[a]);
+      dsq += (double)__fmul_rn(e, e);
+    }
+    if (range_set && dsq > range_sq) return false;
+    if (map_find(t, pack_key(q, cur[0], cur[1], cur[2]), &c) >= 0 && c.lo >= 0.f) return true;
+  }
+}
+
+// The server's render (OctomapServer::render, :193-281; oracle/octomap_server_render.py::render)
+struct RenderParams {
+  const float* points;        // [height*width,3] camera frame, NaN = no depth
+  const int* walk;            // [n_walk] dense indices of the rendered instances, ascending id
+  const double* inst_res;     // [n_inst] resolution of each instance
+  const unsigned* box;        // [n_inst,6] box_enc (k_map_server_boxes)
+  int height, width, n_walk;
+  float m[12];                // rows 0-2 of sensorToWorld as an Eigen::Matrix4f
+  float ox, oy, oz;           // sensor origin (point3d: floats)
+  float fx, fy, cx, cy;       // camera_info K rounded to float (:224-227)
+};
+
+// One thread per (rendered instance w, even pixel e), w-major: a warp is 32 neighbouring rays of
+// one instance.  A pixel with depth casts to its world point, and only into instances whose box
+// holds that point (inBBX, :245); a NaN pixel casts to the z = 1 point of its ray with no box
+// test (:221-237).  maxRange = 1.1 |point - origin|.  The hit distance, a positive float whose
+// bits order like its value, and w pack into one u64 per even pixel: atomicMin keeps the nearest
+// hit, and of exact ties the lowest w, i.e. the lowest instance id (the server on one thread:
+// std::map order and a strict <).
+__global__ void __launch_bounds__(256)
+k_map_render_rays(RenderParams p, MapTable t, u64* __restrict__ zbuf) {
+  const int we = (p.width + 1) >> 1;
+  const long long n_even = (long long)((p.height + 1) >> 1) * we;
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_even * p.n_walk) return;
+  const int w = (int)(g / n_even);
+  const int e = (int)(g - (long long)w * n_even);
+  const int v = 2 * (e / we), u = 2 * (e - (e / we) * we);
+  const size_t i = (size_t)v * p.width + u;
+  const int q = p.walk[w];
+  float pt[3];
+  xform_f32(p.m, p.points[3 * i], p.points[3 * i + 1], p.points[3 * i + 2], pt);
+  if (isnan(pt[0]) || isnan(pt[1]) || isnan(pt[2])) {
+    xform_f32(p.m, __fdiv_rn(__fsub_rn((float)u, p.cx), p.fx),
+              __fdiv_rn(__fsub_rn((float)v, p.cy), p.fy), 1.f, pt);
+  } else {
+    const unsigned* b = p.box + 6 * q;
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+      if (!(pt[a] >= box_dec(b[a]) && pt[a] <= box_dec(b[3 + a]))) return;
+  }
+  const float o[3] = {p.ox, p.oy, p.oz};
+  float dir[3], end[3], de[3];
+  const double range = point_diff_norm(pt, p.ox, p.oy, p.oz, dir) * 1.1;
+  if (!cast_ray(t, q, p.inst_res[q], o, dir, range, end)) return;
+  const float d = (float)point_diff_norm(end, p.ox, p.oy, p.oz, de);
+  atomicMin(zbuf + e, ((u64)__float_as_uint(d) << 32) | (u64)(unsigned)w);
+}
+
+// One thread per pixel: the nearest instance of the even pixel (v, u) labels rows v-1..v and
+// columns u-1..u (the dj, di in {-1, 0} loop, :268-276) and its distance is the depth at (v, u);
+// everything else is `uncertain` / NaN.
+__global__ void __launch_bounds__(256)
+k_map_render_write(const u64* __restrict__ zbuf, const int* __restrict__ walk_ids, int height,
+                   int width, int uncertain, int* __restrict__ label, float* __restrict__ depth) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)height * width) return;
+  const int r = (int)(i / width), c = (int)(i - (long long)r * width);
+  const int v = r + (r & 1), u = c + (c & 1);
+  int lab = uncertain;
+  float d = __uint_as_float(0x7fc00000u);
+  if (v < height && u < width) {
+    const u64 z = zbuf[(size_t)(v >> 1) * ((width + 1) >> 1) + (u >> 1)];
+    if (z != ~0ull) {
+      lab = walk_ids[(unsigned)(z & 0xffffffffull)];
+      if (v == r && u == c) d = __uint_as_float((unsigned)(z >> 32));
+    }
+  }
+  label[i] = lab;
+  depth[i] = d;
+}
+
 __global__ void __launch_bounds__(256)
 k_map_rehash(const MapCell* __restrict__ old, unsigned old_cap, MapTable t) {
   for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < old_cap; i += gridDim.x * blockDim.x) {
@@ -825,13 +1047,14 @@ extern "C" int mf_map_integrate_server(const float* points, const int32_t* label
                                        float lo_min, float lo_max, void* centre_sums,
                                        uint32_t* centre_first, float* centres,
                                        int32_t* centre_set, void* cells, void* cnt,
-                                       int64_t capacity, int32_t* counters, void* stream_) {
+                                       int64_t capacity, int32_t* counters,
+                                       int32_t* tree_state, uint32_t* boxes, void* stream_) {
   const long long n = (long long)height * width;
   if (!points || !labels || !lut || lut_n <= 0 || !inst_resolution || height <= 0 || width <= 0 ||
       n >= (1LL << 31) || n_instances <= 0 || background < 0 || background >= n_instances ||
       !(background_resolution > 0.0) || !xform_ok(sensor_to_world) || isnan(max_range) ||
       !centre_sums || !centre_first || !centres || !centre_set || scan == 0 ||
-      scan >= (1u << 31) || !table_ok(cells, cnt, capacity, counters))
+      scan >= (1u << 31) || !table_ok(cells, cnt, capacity, counters) || !tree_state || !boxes)
     return MF_E_BADARG;
   cudaStream_t st = (cudaStream_t)stream_;
   MapTable t = make_table(cells, cnt, capacity, counters);
@@ -844,7 +1067,12 @@ extern "C" int mf_map_integrate_server(const float* points, const int32_t* label
   p.ox = sensor_to_world[3]; p.oy = sensor_to_world[7]; p.oz = sensor_to_world[11];
   p.max_range = max_range; p.res = background_resolution; p.scan = scan;
   p.hit = hit; p.miss = miss; p.lo_min = lo_min; p.lo_max = lo_max;
+  k_map_server_trees<<<div_up(n, 256), 256, 0, st>>>(p, tree_state, boxes);
+  MF_LAUNCH_CHECK();
   k_map_server_hits<<<div_up(n, 256), 256, 0, st>>>(p, t);
+  MF_LAUNCH_CHECK();
+  k_map_server_boxes<<<div_up(n > n_instances ? n : n_instances, 256), 256, 0, st>>>(
+      p, n_instances, tree_state, boxes);
   MF_LAUNCH_CHECK();
   k_map_scan_free<<<div_up(n, 256), 256, 0, st>>>(p, t);
   MF_LAUNCH_CHECK();
@@ -865,6 +1093,38 @@ extern "C" int mf_map_server_grid_params(const int32_t* target_index, int T,
   k_map_server_grid_params<<<div_up(T, 256), 256, 0, (cudaStream_t)stream_>>>(
       target_index, T, inst_resolution, centres, make_xform(world_to_sensor, 0), off_x, off_y,
       off_z, pitch, origin);
+  MF_LAUNCH_CHECK();
+  return MF_OK;
+}
+
+extern "C" int mf_map_render(const float* points, int height, int width,
+                             const float* sensor_to_world, float fx, float fy, float cx, float cy,
+                             const int32_t* walk, const int32_t* walk_ids, int n_walk,
+                             const double* inst_resolution, const uint32_t* boxes, int uncertain,
+                             void* zbuf, int32_t* label, float* depth, void* cells, void* cnt,
+                             int64_t capacity, int32_t* counters, void* stream_) {
+  const long long n = (long long)height * width;
+  if (!points || height <= 0 || width <= 0 || n >= (1LL << 31) || !xform_ok(sensor_to_world) ||
+      !isfinite(fx) || !isfinite(fy) || !isfinite(cx) || !isfinite(cy) || n_walk < 0 ||
+      n_walk >= 0xFFFF || (n_walk > 0 && (!walk || !walk_ids || !inst_resolution || !boxes)) ||
+      !zbuf || !label || !depth || !table_ok(cells, cnt, capacity, counters))
+    return MF_E_BADARG;
+  cudaStream_t st = (cudaStream_t)stream_;
+  const long long n_even = (long long)((height + 1) / 2) * ((width + 1) / 2);
+  MF_CUDA_TRY(cudaMemsetAsync(zbuf, 0xFF, (size_t)n_even * sizeof(u64), st));
+  if (n_walk > 0) {
+    RenderParams p;
+    p.points = points; p.walk = walk; p.inst_res = inst_resolution; p.box = boxes;
+    p.height = height; p.width = width; p.n_walk = n_walk;
+    for (int a = 0; a < 12; ++a) p.m[a] = sensor_to_world[a];
+    p.ox = sensor_to_world[3]; p.oy = sensor_to_world[7]; p.oz = sensor_to_world[11];
+    p.fx = fx; p.fy = fy; p.cx = cx; p.cy = cy;
+    k_map_render_rays<<<div_up(n_even * n_walk, 256), 256, 0, st>>>(
+        p, make_table(cells, cnt, capacity, counters), (u64*)zbuf);
+    MF_LAUNCH_CHECK();
+  }
+  k_map_render_write<<<div_up(n, 256), 256, 0, st>>>((const u64*)zbuf, walk_ids, height, width,
+                                                     uncertain, label, depth);
   MF_LAUNCH_CHECK();
   return MF_OK;
 }
