@@ -1048,6 +1048,30 @@ int mf_training_transform(int B, const float* grid_target, const float* grid_non
                           const uint64_t* selected, uint8_t* grid_target_out,
                           uint8_t* grid_nontarget_empty_out, void* stream);
 
+/* ------------------------------------------------------------------------
+ * CAD render (geometry.render_cad; the masks and depth of extra/_pybullet.py:215-288
+ * render_cad, each pose rendered alone; oracle/render_cad.py states the rules).
+ * mf_render_cad: N poses of S meshes packed back to back.  vertices [V,3] f64 and faces [F,3]
+ *     int32 (indices into vertices) on the device; offsets [S+1] int64 on the HOST, mesh s is
+ *     faces[offsets[s] .. offsets[s+1]) (offsets[0] = 0, non-decreasing, offsets[S] = F,
+ *     1 <= S <= MF_RENDER_CAD_MAX_MESHES); mesh [N] int32 and Ts_cad2cam [N,4,4] f64 row-major
+ *     on the device.  f = (height / 2) / tan(fovy / 2) in pixels, principal point at the image
+ *     centre.  Writes depth [N,height,width] f32 (NaN where nothing covers), mask [N,height,width]
+ *     u8 0/1 and count [N] int32 (mask pixels).  A face with a vertex index outside [0, V) is
+ *     dropped (the binding rejects such faces on the host before upload); a pose whose mesh index
+ *     is outside [0, S) renders nothing.  Three launches, no host read, no memset; outputs are
+ *     bitwise identical between runs.  MF_E_BADARG, before any launch, for height or width <= 0,
+ *     height * width >= 2^30, N, F or V < 0, bad offsets, f not finite and positive, or a NULL
+ *     pointer the call needs; N = 0 returns MF_OK without a launch.  workspace:
+ *     mf_render_cad_workspace_bytes(N, F, height, width) bytes, no initial contents.
+ * ------------------------------------------------------------------------ */
+#define MF_RENDER_CAD_MAX_MESHES 64
+size_t mf_render_cad_workspace_bytes(int N, int F, int height, int width);
+int mf_render_cad(const double* vertices, int V, const int32_t* faces, int F,
+                  const int64_t* offsets, int S, const int32_t* mesh, const double* Ts_cad2cam,
+                  int N, double f, int height, int width, float* depth, uint8_t* mask,
+                  int32_t* count, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -159,6 +159,9 @@ SIGNATURES = {
     "mf_training_full_grids": (c_i, [c_i, c_p, c_p, c_p, c_i, c_p, c_p, c_p, c_p, c_p, c_p]),
     "mf_training_nontarget_present": (c_i, [c_i, c_p, c_p, c_p]),
     "mf_training_transform": (c_i, [c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),
+    "mf_render_cad_workspace_bytes": (c_sz, [c_i, c_i, c_i, c_i]),
+    "mf_render_cad": (c_i, [c_p, c_i, c_p, c_i, c_p, c_i, c_p, c_p, c_i, c_d, c_i, c_i, c_p, c_p,
+                            c_p, c_p, c_sz, c_p]),
 }
 
 _lib = None

@@ -47,6 +47,7 @@ SOURCES = {
     "icp_link.cu": ["-fmad=false"],
     "pose_metrics.cu": ["-fmad=false"],
     "training_examples.cu": ["-fmad=false"],
+    "render_cad.cu": ["-fmad=false"],
 }
 
 

@@ -77,7 +77,7 @@ def empty_examples(dev, D, S):
 
 def build_examples(rgb, depth, K, label, instance_ids, class_ids, pitch_table, mapping=None, *,
                    dev, n_points_minimal=1, dimensions=32, image_size=256, class_filter=None,
-                   sensor_to_world=None):
+                   sensor_to_world=None, with_n_mask=False):
     """The model-free part of an example of every instance of one labelled frame, as get_example
     builds it (datasets/rgbd_pose_estimation/base.py:78-197) and the pose node (ros/src/
     morefusion_ros/nodes/singleview_3d_pose_estimation.py:113-185) around it: the map, the
@@ -107,8 +107,11 @@ def build_examples(rgb, depth, K, label, instance_ids, class_ids, pitch_table, m
     without a server centre yet is skipped; origin is the server's grid origin rounded to
     float32, pitch the server's, and the three map grids are replaced by grid_nontarget_empty
     [M,D,D,D] bool, the server's grid_noentry > 0.  The "set" flags of the centres travel in the
-    one host read."""
-    ids = np.asarray(instance_ids).reshape(-1)
+    one host read.
+
+    with_n_mask: the examples of kept instances also hold n_mask [M] int32, each one's
+    label-mask pixel count (a gather of the crop pass's counts, no host read)."""
+    ids =np.asarray(instance_ids).reshape(-1)
     cls = np.asarray(class_ids).reshape(-1).astype(np.int64)
     if ids.shape != cls.shape:
         raise ValueError("instance_ids and class_ids must have the same length")
@@ -158,6 +161,8 @@ def build_examples(rgb, depth, K, label, instance_ids, class_ids, pitch_table, m
     ex = dict(class_id=_util.h2d(cls_kept, dev, torch.int32, "frame/class"),
               rgb=rgb_ins.index_select(0, kd), pcd=pcd_ins.index_select(0, kd),
               instance_ids=kept_ids, index=np.flatnonzero(fg)[k])
+    if with_n_mask:
+        ex["n_mask"] = stats[:, 4].index_select(0, kd)
     if server:
         # the node's decoding of grids_noentry (:131-148): every listed index is True, the
         # origin a float32 array of the message's float64 origin

@@ -59,22 +59,27 @@ def full_grids(points, offsets, seg, R, t, origin, pitch, d_offsets=None):
 
 
 class RGBDPoseEstimationDatasetBase:
-    """RGBDPoseEstimationDatasetBase(models, class_ids=None): subclasses implement ``get_frame``
+    """RGBDPoseEstimationDatasetBase(models, class_ids=None, with_visibility=False): subclasses implement ``get_frame``
     (a dict with instance_ids [N], class_ids [N], rgb [H,W,3] uint8, depth [H,W] float metres,
     instance_label [H,W], intrinsic_matrix [3,3] and Ts_cad2cam [N,4,4]) and ``__len__``.
 
     models: ``get_voxel_pitch(dimension, class_id)`` and ``get_solid_voxel_grid(class_id)``
     (an object with ``.points`` [n,3], the solid voxel centres in the CAD frame).  class_ids:
     the classes an example may have (the others still go into the map).  device: where the
-    examples are built (the current CUDA device when None)."""
+    examples are built (the current CUDA device when None).  with_visibility: examples also hold
+    ``visibility`` (``get_example``), which needs ``models.get_cad(class_id)`` (an object with
+    ``.vertices`` [V,3] and ``.faces`` [F,3]); off by default, as in the reindexed datasets that
+    training uses (reindexed.py:159-160 drop it)."""
 
     _n_points_minimal = 1
     _image_size = 256
     _voxel_dim = VOXEL_DIM
     _n_fg_class = 21
 
-    def __init__(self, models, class_ids=None, device=None):
+    def __init__(self, models, class_ids=None, device=None, with_visibility=False):
         self._models = models
+        self._with_visibility = bool(with_visibility)
+        self._cad_cache = {}
         self._class_ids = tuple(class_ids) if class_ids is not None else None
         self._device = torch.device(device) if device is not None else None
         self._pitch_table = np.array(
@@ -104,6 +109,41 @@ class RGBDPoseEstimationDatasetBase:
                 _util.h2d_transient(offsets, dev, torch.int64))
         return self._solid_cache[key]
 
+    def _cad_table(self, dev):
+        """Every class's CAD mesh back to back on the device (checked on the host and uploaded
+        once): vertices [V,3] float64, faces [F,3] int32 indexing the packed vertices, and the
+        host int64 face offsets [n_fg_class + 1] (class c is mesh c - 1)."""
+        key = str(dev)
+        if key not in self._cad_cache:
+            vs, fs, offsets, base = [], [], [0], 0
+            for c in range(1, self._n_fg_class + 1):
+                cad = self._models.get_cad(c)
+                v, f = geometry._check_mesh(cad.vertices, cad.faces)
+                vs.append(v)
+                fs.append(f + base)
+                base += len(v)
+                offsets.append(offsets[-1] + len(f))
+            self._cad_cache[key] = (
+                _util.h2d_transient(np.concatenate(vs), dev, torch.float64),
+                _util.h2d_transient(np.concatenate(fs), dev, torch.int32),
+                np.asarray(offsets, np.int64))
+        return self._cad_cache[key]
+
+    def _visibility(self, ex, cls_kept, Ts, K, height, width, dev):
+        """visibility [M] float64: each kept instance's label-mask pixel count over the pixel
+        count of its CAD model rendered alone at Ts_cad2cam (base.py:139-148), every instance in
+        one render call; 0/0 gives NaN and x/0 inf, as NumPy does under the reference's
+        errstate."""
+        n_mask = ex.pop("n_mask")
+        if len(cls_kept) == 0:
+            return torch.empty(0, dtype=torch.float64, device=dev)
+        vertices, faces, offsets = self._cad_table(dev)
+        fovy = geometry.fovy_from_intrinsics(K[1, 1], height)
+        _, _, count = geometry._render_cad_batch(
+            vertices, faces, offsets, cls_kept.astype(np.int32) - 1, Ts,
+            f=geometry.focal_from_fovy(fovy, height), height=height, width=width)
+        return n_mask.to(torch.float64) / count.to(torch.float64)
+
     def get_example(self, index):
         """The kept instances of frame ``index`` as one batched dict of CUDA tensors, with
         get_example's keys except visibility: class_id [M] int32, rgb [M,256,256,3] uint8, pcd
@@ -111,9 +151,10 @@ class RGBDPoseEstimationDatasetBase:
         (quaternion_from_matrix / translation_from_matrix of Ts_cad2cam), origin [M,3] float32,
         pitch [M] float64, grid_target / grid_nontarget / grid_empty [M,32,32,32] float32 as the
         map query returns them, grid_target_full / grid_nontarget_full [M,32,32,32] int32
-        (``full_grids``); and instance_ids [M] (numpy).  The keep rules are the reference's
+        (``full_grids``); and instance_ids [M] (numpy).  With ``with_visibility``, also
+        visibility [M] float64 (``_visibility``).  The keep rules are the reference's
         (``build_examples``).  Host reads: those of ``build_examples`` with the map built from the
-        frame; the full grids add none."""
+        frame; the full grids and the visibility add none."""
         frame = self.get_frame(index)
         dev = self._dev()
         D = self._voxel_dim
@@ -126,7 +167,10 @@ class RGBDPoseEstimationDatasetBase:
             ex, cls_kept, _ = build_examples(
                 frame["rgb"], frame["depth"], frame["intrinsic_matrix"], frame["instance_label"],
                 ids, cls, self._pitch_table, dev=dev, n_points_minimal=self._n_points_minimal,
-                dimensions=D, image_size=self._image_size, class_filter=self._class_ids or None)
+                dimensions=D, image_size=self._image_size, class_filter=self._class_ids or None,
+                with_n_mask=self._with_visibility)
+        if self._with_visibility and "n_mask" not in ex:
+            ex["n_mask"] = torch.empty(0, dtype=torch.int32, device=dev)
         Ts = Ts[ex.pop("index")]
         q = np.zeros((len(Ts), 4))
         R = np.zeros((len(Ts), 3, 3))
@@ -141,15 +185,21 @@ class RGBDPoseEstimationDatasetBase:
         ex["translation_true"] = _util.h2d(t, dev, torch.float64, "example/t")
         ex["grid_target_full"] = gtf
         ex["grid_nontarget_full"] = gnf
+        if self._with_visibility:
+            H, W = np.shape(frame["instance_label"])[:2]
+            ex["visibility"] = self._visibility(
+                ex, cls_kept, Ts, np.asarray(frame["intrinsic_matrix"], np.float64).reshape(3, 3),
+                H, W, dev)
         return ex
 
 
 class SyntheticRGBDPoseEstimationDataset(RGBDPoseEstimationDatasetBase):
     """Frames of ``synthetic.make_pose_frame``: frame i is seed ``seed + i``."""
 
-    def __init__(self, size, seed=0, n_objects=8, class_ids=None, models=None, device=None):
+    def __init__(self, size, seed=0, n_objects=8, class_ids=None, models=None, device=None,
+                 with_visibility=False):
         super().__init__(synthetic.SyntheticYCBModels() if models is None else models,
-                         class_ids=class_ids, device=device)
+                         class_ids=class_ids, device=device, with_visibility=with_visibility)
         self._size = int(size)
         self._seed = int(seed)
         self._n_objects = int(n_objects)

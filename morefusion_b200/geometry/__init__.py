@@ -231,3 +231,126 @@ def instance_crops(rgb, pcd, label, instance_ids, *, size=256):
     if is_np:
         out = tuple(o.cpu().numpy() for o in out)
     return out
+
+
+def _check_faces(faces, n_vertices):
+    """Host check of a mesh's faces before upload: [F,3] integer indices in [0, n_vertices),
+    returned as int32."""
+    f = np.asarray(faces)
+    if f.size and not np.issubdtype(f.dtype, np.integer):
+        raise ValueError("faces must be integer vertex indices")
+    f = f.reshape(-1, 3).astype(np.int64)
+    if f.size and (f.min() < 0 or f.max() >= n_vertices):
+        raise ValueError("face index outside [0, len(vertices))")
+    return np.ascontiguousarray(f.astype(np.int32))
+
+
+def _check_mesh(vertices, faces):
+    """Host checks of a mesh before upload: vertices [V,3] float64, faces [F,3] int32 in [0, V)."""
+    v = np.ascontiguousarray(np.asarray(vertices, dtype=np.float64).reshape(-1, 3))
+    return v, _check_faces(faces, len(v))
+
+
+def focal_from_fovy(fovy, height):
+    """The focal length in pixels of computeProjectionMatrixFOV's frustum of vertical field of
+    view ``fovy`` degrees over ``height`` rows (float64)."""
+    import math
+    return (height / 2.0) / math.tan(math.radians(float(fovy)) / 2.0)
+
+
+def fovy_from_intrinsics(fy, height):
+    """The vertical field of view in degrees that trimesh.scene.Camera(resolution=(W, H),
+    focal=(fx, fy)).fov[1] gives, as get_example passes it to render_cad."""
+    return float(2.0 * np.degrees(np.arctan(height / (2.0 * float(fy)))))
+
+
+def _render_cad_batch(vertices, faces, offsets, mesh, Ts_cad2cam, *, f, height, width):
+    """N poses of S meshes packed back to back, each pose rendered alone (csrc/render_cad.cu).
+
+    vertices [V,3] float64 and faces [F,3] int32 CUDA tensors, already checked on the host
+    (``_check_mesh``; face indices of mesh s index the packed vertices); offsets [S+1] host
+    int64, mesh s is faces[offsets[s]:offsets[s+1]]; mesh [N] (the mesh of each pose) and
+    Ts_cad2cam [N,4,4] float64 CUDA tensors or host arrays (uploaded without a host sync); f
+    the focal length in pixels.  Returns CUDA tensors depth [N,H,W] float32 (NaN where nothing
+    covers), mask [N,H,W] bool and count [N] int32.  Three launches, no host read."""
+    import torch
+    from .. import _lib
+    from ..functions.geometry import _util
+    _lib.require_cuda(vertices, faces)
+    dev = vertices.device
+    offsets = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1))
+    d_mesh = _util.h2d(mesh, dev, torch.int32, "render_cad/mesh").contiguous()
+    d_T = _util.h2d(Ts_cad2cam, dev, torch.float64, "render_cad/T").contiguous()
+    N = d_mesh.numel()
+    if tuple(d_T.shape) != (N, 4, 4):
+        raise ValueError("Ts_cad2cam must be [N,4,4] with one mesh index per pose")
+    H, W = int(height), int(width)
+    depth = torch.empty((N, H, W), dtype=torch.float32, device=dev)
+    mask = torch.empty((N, H, W), dtype=torch.bool, device=dev)
+    count = torch.empty(N, dtype=torch.int32, device=dev)
+    L = _lib.lib()
+    F = faces.shape[0]
+    ws_bytes = L.mf_render_cad_workspace_bytes(N, F, H, W)
+    ws = _util.workspace(ws_bytes, dev) if ws_bytes else None
+    with torch.cuda.device(dev):
+        _lib.check(L.mf_render_cad(
+            _lib.ptr(vertices), vertices.shape[0], _lib.ptr(faces), F,
+            offsets.ctypes.data_as(_lib.ctypes.c_void_p), offsets.size - 1, _lib.ptr(d_mesh),
+            _lib.ptr(d_T), N, float(f), H, W, _lib.ptr(depth), _lib.ptr(mask.view(torch.uint8)),
+            _lib.ptr(count), _lib.ptr(ws), ws_bytes, _lib.stream()), "render_cad")
+    return depth, mask, count
+
+
+def render_cad(vertices, faces, Ts_cad2cam, *, fovy, height, width):
+    """Depth and mask of a CAD mesh at one pose [4,4] or N poses [N,4,4], each pose rendered
+    alone, as morefusion/extra/_pybullet.py:215-288 ``render_cad`` renders them with pybullet.
+
+    The reference takes a mesh file; here the caller passes the mesh: vertices [V,3] and faces
+    [F,3] integer indices (a loaded ``trimesh.Trimesh`` passes ``.vertices`` and ``.faces``).
+    Ts_cad2cam maps CAD points into the camera frame (OpenCV axes).  The camera is pybullet's
+    computeProjectionMatrixFOV(fovy, W / H, 0.01, 1000): square pixels of focal length
+    (H / 2) / tan(fovy / 2) and the principal point at the image centre.  RGB is not produced:
+    textures are out of scope.
+
+    Returns (depth, mask): depth float32 camera-frame Z of the nearest surface, NaN where the
+    mesh does not cover; mask bool, the covered pixels; [H,W] for one pose, [N,H,W] for N
+    poses.  NumPy in gives NumPy out; CUDA tensors in give CUDA tensors out.  The rasterisation
+    rules (snapping, fill rule, triangles crossing the near plane) are DESIGN's render_cad
+    section.  Faces are checked on the host, so CUDA faces are read back once."""
+    import torch
+    from .. import _lib
+    from ..functions.geometry import _util
+    is_np = not isinstance(vertices, torch.Tensor)
+    if is_np:
+        v, fc = _check_mesh(vertices, faces)
+        dev = torch.device("cuda", torch.cuda.current_device())
+    else:
+        _lib.require_cuda(vertices)
+        dev = vertices.device
+        v = None
+        fc = _check_faces(faces.cpu().numpy() if isinstance(faces, torch.Tensor) else faces,
+                          vertices.shape[0])
+    Ts = Ts_cad2cam
+    if isinstance(Ts, torch.Tensor):
+        _lib.require_cuda(Ts)
+        squeeze = Ts.dim() == 2
+        Ts = Ts.to(torch.float64).reshape(-1, 4, 4).contiguous()
+    else:
+        Ts = np.asarray(Ts, np.float64)
+        squeeze = Ts.ndim == 2
+        Ts = Ts.reshape(-1, 4, 4)
+    height, width = int(height), int(width)
+    f = focal_from_fovy(fovy, height)
+    if not (np.isfinite(f) and f > 0):
+        raise ValueError("fovy must be in (0, 180) degrees")
+    d_v = (_util.h2d_transient(v, dev, torch.float64) if is_np
+           else vertices.to(torch.float64).contiguous())
+    d_f = _util.h2d_transient(fc, dev, torch.int32)
+    N = Ts.shape[0]
+    depth, mask, _ = _render_cad_batch(d_v, d_f, [0, len(fc)], np.zeros(N, np.int32), Ts,
+                                       f=f, height=height, width=width)
+    if squeeze:
+        depth, mask = depth[0], mask[0]
+    if is_np:
+        return depth.cpu().numpy(), mask.cpu().numpy()
+    return depth, mask

@@ -158,6 +158,17 @@ class SyntheticYCBModels:
     def get_sdf(self, class_id):
         return sdf_lattice(int(class_id), self._kinds)
 
+    def get_cad(self, class_id):
+        """Stand-in for YCBVideoModels.get_cad (models.py:88-94, the loaded trimesh of
+        textured_simple.obj): an object with ``.vertices`` [V,3] float64 and ``.faces`` [F,3]
+        int32, a closed triangulation of the class primitive with every vertex on its surface and
+        the faces wound outward.  A box is its 12 triangles; a cylinder has 32 segments around
+        (two rings and a centre on each cap: 66 vertices, 128 faces); a sphere has 16 rings of
+        latitude and 32 segments of longitude (two poles and 15 rings: 482 vertices, 960 faces)."""
+        kind, half = _primitive(int(class_id), self._kinds)
+        v, f = cad_mesh(kind, half)
+        return types.SimpleNamespace(vertices=v, faces=f)
+
     def get_solid_voxel_grid(self, class_id):
         """Stand-in for YCBVideoModels.get_solid_voxel_grid (models.py:81-86, a binvox of the CAD
         model): an object whose ``.points`` [n,3] float64 are the lattice points inside the class
@@ -169,6 +180,40 @@ class SyntheticYCBModels:
         ax = [np.arange(-np.floor(h / pitch), np.floor(h / pitch) + 1) * pitch for h in half]
         g = np.stack(np.meshgrid(*ax, indexing="ij"), -1).reshape(-1, 3)
         return types.SimpleNamespace(points=g[sdf_primitive(kind, half, g) >= 0], pitch=pitch)
+
+
+def cad_mesh(kind, half, n_around=32, n_rings=16):
+    """(vertices [V,3] float64, faces [F,3] int32) of the primitive, as ``get_cad`` states."""
+    if kind == "box":
+        v = np.array([[x, y, z] for x in (-1, 1) for y in (-1, 1) for z in (-1, 1)], np.float64) * half
+        quads = [(0, 1, 3, 2), (4, 6, 7, 5), (0, 4, 5, 1), (2, 3, 7, 6), (0, 2, 6, 4), (1, 5, 7, 3)]
+        f = [t for a, b, c, d in quads for t in ((a, b, c), (a, c, d))]
+        return v, np.array(f, np.int32)
+    phi = 2 * np.pi * np.arange(n_around) / n_around
+    ring = np.stack([np.cos(phi), np.sin(phi)], 1)
+    j = np.arange(n_around)
+    k = (j + 1) % n_around
+    if kind == "cylinder":
+        r, h = half[0], half[2]
+        v = np.concatenate([np.c_[r * ring, np.full(n_around, -h)], np.c_[r * ring, np.full(n_around, h)],
+                            [[0.0, 0.0, -h], [0.0, 0.0, h]]])
+        lo, hi, cb, ct = 0, n_around, 2 * n_around, 2 * n_around + 1
+        f = np.concatenate([np.c_[lo + j, lo + k, hi + k], np.c_[lo + j, hi + k, hi + j],
+                            np.c_[np.full(n_around, cb), lo + k, lo + j],
+                            np.c_[np.full(n_around, ct), hi + j, hi + k]])
+        return v, f.astype(np.int32)
+    r = half[0]
+    theta = np.pi * np.arange(1, n_rings) / n_rings
+    body = np.concatenate([np.c_[r * np.sin(t) * ring, np.full(n_around, r * np.cos(t))] for t in theta])
+    v = np.concatenate([[[0.0, 0.0, r]], body, [[0.0, 0.0, -r]]])
+    south = len(v) - 1
+    f = [np.c_[np.zeros(n_around, int), 1 + j, 1 + k]]
+    for i in range(n_rings - 2):
+        a, b = 1 + i * n_around, 1 + (i + 1) * n_around
+        f += [np.c_[a + j, b + j, b + k], np.c_[a + j, b + k, a + k]]
+    a = 1 + (n_rings - 2) * n_around
+    f.append(np.c_[np.full(n_around, south), a + k, a + j])
+    return v, np.concatenate(f).astype(np.int32)
 
 
 def sdf_lattice(class_id, kinds=("box", "cylinder", "sphere")):
