@@ -179,22 +179,24 @@ def _keys(tree, pts):
     return (k[:, 0] << 32) | (k[:, 1] << 16) | k[:, 2], ok
 
 
-def ray_keys(tree, origin, ends):
+def ray_keys(tree, origin, ends, counts=False):
     """The union of ``OcTree.computeRayKeys(origin, end)`` (oracle/octomap.py, first cell
     included, end cell excluded, nothing for a ray with an end outside the key range) over the
     rows of ends [N, 3] float32, as packed int64 keys: the same arithmetic, every ray stepped in
-    lockstep."""
+    lockstep.  counts: also the number of rays whose key list holds each key (a ray never
+    crosses a cell twice), as (keys, counts)."""
     origin = np.asarray(origin, np.float32)
     ends = np.asarray(ends, np.float32).reshape(-1, 3)
+    none = (np.empty(0, np.int64), np.empty(0, np.int64)) if counts else np.empty(0, np.int64)
     ko, ok_o = _keys(tree, origin[None])
     if not ok_o[0] or not len(ends):
-        return np.empty(0, np.int64)
+        return none
     ke, ok_e = _keys(tree, ends)
     act = ok_e & (ke != ko[0])
     ends, ke = ends[act], ke[act]
     if not len(ends):
-        return np.empty(0, np.int64)
-    out = [np.full(1, ko[0])]
+        return none
+    out = [np.full(len(ends) if counts else 1, ko[0])]
     res = tree.resolution
     d = (ends - origin).astype(np.float32)
     nsq = ((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2]).astype(np.float32)
@@ -228,7 +230,7 @@ def ray_keys(tree, origin, ends):
         out.append((c[:, 0] << 32) | (c[:, 1] << 16) | c[:, 2])
         cur, tmax, tdelta, step, kend, flen = cur[go], tmax[go], tdelta[go], step[go], kend[go], flen[go]
         rows = rows[go]
-    return np.unique(np.concatenate(out))
+    return np.unique(np.concatenate(out), return_counts=counts)
 
 
 def centre(points):
