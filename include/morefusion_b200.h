@@ -1072,6 +1072,28 @@ int mf_render_cad(const double* vertices, int V, const int32_t* faces, int F,
                   int N, double f, int height, int width, float* depth, uint8_t* mask,
                   int32_t* count, void* workspace, size_t workspace_bytes, void* stream);
 
+/* mf_render_scene (geometry.render_instances; the depth and instance image of the picking-order
+ *     node's _render_object_pose_array, ros/.../select_picking_order.py:129-190): N posed objects
+ *     rendered together into one camera.  Meshes, mesh [N], Ts_cad2cam [N,4,4], f and the
+ *     argument checks are those of mf_render_cad, and each object's coverage and depth are the
+ *     bits mf_render_cad gives it alone.  instance_ids [N] int32 on the device.  The visible
+ *     object of a pixel is the one of smallest float32 depth; an exact tie goes to the lower
+ *     index.  Writes depth [height,width] f32 (NaN where nothing covers), ins [height,width]
+ *     int32 (instance_ids of the visible object, -1 where nothing covers), whole [N] int32 (the
+ *     pixels each object covers alone, = mf_render_cad's count) and occluded [N,N] int32
+ *     (occluded[i][j]: pixels object i covers where object j is visible; zero diagonal).  Four
+ *     launches, no host read, no memset; outputs are bitwise identical between runs.
+ *     N > MF_RENDER_SCENE_MAX_OBJECTS returns MF_E_UNSUPPORTED before any launch.  N = 0 writes
+ *     the empty image (NaN / -1) in one launch; mesh, Ts_cad2cam, instance_ids, whole, occluded
+ *     and workspace may then be NULL.  workspace: mf_render_cad_workspace_bytes(N, F, height,
+ *     width) bytes, no initial contents. */
+#define MF_RENDER_SCENE_MAX_OBJECTS 64
+int mf_render_scene(const double* vertices, int V, const int32_t* faces, int F,
+                    const int64_t* offsets, int S, const int32_t* mesh, const double* Ts_cad2cam,
+                    const int32_t* instance_ids, int N, double f, int height, int width,
+                    float* depth, int32_t* ins, int32_t* whole, int32_t* occluded,
+                    void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -162,6 +162,8 @@ SIGNATURES = {
     "mf_render_cad_workspace_bytes": (c_sz, [c_i, c_i, c_i, c_i]),
     "mf_render_cad": (c_i, [c_p, c_i, c_p, c_i, c_p, c_i, c_p, c_p, c_i, c_d, c_i, c_i, c_p, c_p,
                             c_p, c_p, c_sz, c_p]),
+    "mf_render_scene": (c_i, [c_p, c_i, c_p, c_i, c_p, c_i, c_p, c_p, c_p, c_i, c_d, c_i, c_i, c_p,
+                              c_p, c_p, c_p, c_p, c_sz, c_p]),
 }
 
 _lib = None

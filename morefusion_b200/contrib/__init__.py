@@ -8,3 +8,4 @@ from .occupancy_registration import OccupancyRegistration  # noqa: F401  (SURVEY
 from .multi_instance_octree_mapping import MultiInstanceOctreeMapping  # noqa: F401  (SURVEY.md 8f-3)
 from .object_mapping import ObjectMapping  # noqa: F401  (ros/.../nodes/object_mapping.py)
 from .icp_registration import ICPRegistration  # noqa: F401  (ros/.../singleview_3d_pose_estimation.py:246-264)
+from .picking_order import SelectPickingOrder  # noqa: F401  (ros/.../nodes/select_picking_order.py)

@@ -262,6 +262,109 @@ __global__ void __launch_bounds__(RC_THREADS) k_rc_raster(RcParams p, const RcBo
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// One scene of N <= 64 posed objects rendered together (mf_render_scene).  k_rc_init and
+// k_rc_setup build the same records as mf_render_cad; k_rs_zero clears occluded [N,N].
+// k_rs_raster  one CTA per 16x16 tile, a thread per pixel.  The objects are taken in input order;
+//              one whose box misses the tile is skipped.  Each object's faces stream through
+//              shared memory as in k_rc_raster, so rc_cover gives the pixel exactly the coverage
+//              and depth that object has rendered alone.  The pixel keeps a 64-bit cover mask,
+//              the best depth and the best object; only a strict < replaces the best, so an exact
+//              tie goes to the lower index (GL_LESS with the objects drawn in input order).
+//              __syncthreads_count adds each object's covered pixels to whole[n] (= mf_render_cad's
+//              count).  For a pixel whose visible object is j, every other covering object i adds
+//              1 to the tile's occ[i][j] in shared memory; the non-zero entries go to
+//              occluded [N,N] with integer atomics.
+// Every output is a min, a union or an integer sum, so every output is bitwise identical between
+// runs.
+// ------------------------------------------------------------------------------------------
+__global__ void k_rs_zero(int n, int32_t* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = 0;
+}
+
+__global__ void __launch_bounds__(RC_THREADS) k_rs_raster(RcParams p, const RcBox* __restrict__ boxes,
+                                                           const RcGeom* __restrict__ geom,
+                                                           const int4* __restrict__ pose_box,
+                                                           const int32_t* __restrict__ instance_ids,
+                                                           float* __restrict__ depth,
+                                                           int32_t* __restrict__ ins,
+                                                           int32_t* __restrict__ whole,
+                                                           int32_t* __restrict__ occluded) {
+  __shared__ RcGeom s_geom[RC_THREADS];
+  __shared__ RcBox s_box[RC_THREADS];
+  __shared__ int s_occ[MF_RENDER_SCENE_MAX_OBJECTS * MF_RENDER_SCENE_MAX_OBJECTS];
+  __shared__ int s_n;
+  const int tiles_x = (p.W + RC_TILE - 1) / RC_TILE;
+  const int tx0 = (blockIdx.x % tiles_x) * RC_TILE, ty0 = (blockIdx.x / tiles_x) * RC_TILE;
+  const int col = tx0 + (threadIdx.x % RC_TILE), row = ty0 + (threadIdx.x / RC_TILE);
+  const bool on_image = col < p.W && row < p.H;
+  const int tx1 = tx0 + RC_TILE - 1, ty1 = ty0 + RC_TILE - 1;
+  const int NN = p.N * p.N;
+  for (int i = threadIdx.x; i < NN; i += RC_THREADS) s_occ[i] = 0;
+  unsigned long long cover = 0ull;
+  float best = 0.0f;
+  int best_n = -1;
+  for (int n = 0; n < p.N; ++n) {
+    const int4 pb = pose_box[n];
+    int lo, hi;
+    if (!(pb.x <= tx1 && pb.z >= tx0 && pb.y <= ty1 && pb.w >= ty0) || !rc_pose_mesh(p, n, lo, hi))
+      continue;                                      // uniform over the CTA
+    bool hit = false;
+    float zmin = 0.0f;
+    const RcBox* bn = boxes + (size_t)n * p.F;
+    const RcGeom* gn = geom + (size_t)n * p.F;
+    for (int base = lo; base < hi; base += RC_THREADS) {
+      if (threadIdx.x == 0) s_n = 0;
+      __syncthreads();
+      const int k = base + threadIdx.x;
+      if (k < hi) {
+        const RcBox b = bn[k];
+        if (b.x0 <= tx1 && b.x1 >= tx0 && b.y0 <= ty1 && b.y1 >= ty0) {
+          const int slot = atomicAdd(&s_n, 1);        // slot order is free: union and min commute
+          s_box[slot] = b;
+          s_geom[slot] = gn[k];
+        }
+      }
+      __syncthreads();
+      const int m = s_n;
+      if (on_image)
+        for (int q = 0; q < m; ++q) {
+          const RcBox& b = s_box[q];
+          if (col >= b.x0 && col <= b.x1 && row >= b.y0 && row <= b.y1)
+            rc_cover(s_geom[q], col, row, hit, zmin);
+        }
+      __syncthreads();
+    }
+    if (hit) {
+      cover |= 1ull << n;
+      if (best_n < 0 || zmin < best) {
+        best = zmin;
+        best_n = n;
+      }
+    }
+    const int c = __syncthreads_count(hit);
+    if (threadIdx.x == 0 && c > 0) atomicAdd(whole + n, c);
+  }
+  if (on_image) {
+    const size_t o = (size_t)row * p.W + col;
+    depth[o] = best_n >= 0 ? best : __int_as_float(0x7fc00000);
+    ins[o] = best_n >= 0 ? instance_ids[best_n] : -1;
+  }
+  __syncthreads();                                   // s_occ cleared (also when no object ran)
+  if (best_n >= 0) {
+    unsigned long long rest = cover & ~(1ull << best_n);
+    while (rest) {
+      const int i = __ffsll((long long)rest) - 1;
+      rest &= rest - 1;
+      atomicAdd(&s_occ[i * p.N + best_n], 1);
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < NN; i += RC_THREADS)
+    if (s_occ[i]) atomicAdd(occluded + i, s_occ[i]);
+}
+
 #endif  // !MF_HOST_EMU
 
 }  // namespace mf
@@ -316,6 +419,58 @@ extern "C" int mf_render_cad(const double* vertices, int V, const int32_t* faces
   const long long tiles = (long long)div_up(width, RC_TILE) * div_up(height, RC_TILE);
   k_rc_raster<<<dim3((unsigned)tiles, (unsigned)(N < 65535 ? N : 65535)), RC_THREADS, 0, st>>>(
       p, boxes, geom, pose_box, depth, mask, count);
+  MF_LAUNCH_CHECK();
+  return MF_OK;
+}
+
+extern "C" int mf_render_scene(const double* vertices, int V, const int32_t* faces, int F,
+                               const int64_t* offsets, int S, const int32_t* mesh,
+                               const double* Ts_cad2cam, const int32_t* instance_ids, int N,
+                               double f, int height, int width, float* depth, int32_t* ins,
+                               int32_t* whole, int32_t* occluded, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
+  if (height <= 0 || width <= 0 || (long long)height * width >= (1LL << 30)) return MF_E_BADARG;
+  if (N < 0 || F < 0 || V < 0 || S < 1 || S > MF_RENDER_CAD_MAX_MESHES || !offsets)
+    return MF_E_BADARG;
+  if (N > MF_RENDER_SCENE_MAX_OBJECTS) return MF_E_UNSUPPORTED;
+  if (!(f > 0.0) || !isfinite(f)) return MF_E_BADARG;
+  if (offsets[0] != 0 || offsets[S] != F) return MF_E_BADARG;
+  int f_max = 0;
+  for (int s = 0; s < S; ++s) {
+    if (offsets[s + 1] < offsets[s]) return MF_E_BADARG;
+    if (offsets[s + 1] - offsets[s] > f_max) f_max = (int)(offsets[s + 1] - offsets[s]);
+  }
+  if (F > 0 && (!vertices || !faces || V == 0)) return MF_E_BADARG;
+  if (!depth || !ins) return MF_E_BADARG;
+  if (N > 0) {
+    if (!mesh || !Ts_cad2cam || !instance_ids || !whole || !occluded || !workspace)
+      return MF_E_BADARG;
+    if (workspace_bytes < mf_render_cad_workspace_bytes(N, F, height, width)) return MF_E_WORKSPACE;
+  }
+  RcParams p;
+  p.v = vertices; p.faces = faces; p.mesh = mesh; p.T = Ts_cad2cam;
+  p.V = V; p.F = F; p.N = N; p.S = S; p.H = height; p.W = width; p.f_max = f_max; p.f = f;
+  for (int s = 0; s <= S; ++s) p.off[s] = (int)offsets[s];
+  const size_t rec = (size_t)N * F;
+  char* ws = (char*)workspace;
+  RcBox* boxes = (RcBox*)ws;
+  RcGeom* geom = (RcGeom*)(ws + rc_align(rec * sizeof(RcBox)));
+  int4* pose_box = (int4*)(ws + rc_align(rec * sizeof(RcBox)) + rc_align(rec * sizeof(RcGeom)));
+  cudaStream_t st = (cudaStream_t)stream_;
+  if (N > 0) {
+    k_rc_init<<<div_up(N, 128), 128, 0, st>>>(N, pose_box, whole);
+    MF_LAUNCH_CHECK();
+    k_rs_zero<<<div_up(N * N, 256), 256, 0, st>>>(N * N, occluded);
+    MF_LAUNCH_CHECK();
+    if (f_max > 0) {
+      k_rc_setup<<<div_up((long long)N * f_max, RC_THREADS), RC_THREADS, 0, st>>>(p, boxes, geom,
+                                                                                 pose_box);
+      MF_LAUNCH_CHECK();
+    }
+  }
+  const long long tiles = (long long)div_up(width, RC_TILE) * div_up(height, RC_TILE);
+  k_rs_raster<<<(unsigned)tiles, RC_THREADS, 0, st>>>(p, boxes, geom, pose_box, instance_ids,
+                                                      depth, ins, whole, occluded);
   MF_LAUNCH_CHECK();
   return MF_OK;
 }

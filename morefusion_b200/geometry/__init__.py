@@ -354,3 +354,126 @@ def render_cad(vertices, faces, Ts_cad2cam, *, fovy, height, width):
     if is_np:
         return depth.cpu().numpy(), mask.cpu().numpy()
     return depth, mask
+
+
+MAX_SCENE_OBJECTS = 64                    # MF_RENDER_SCENE_MAX_OBJECTS
+
+
+def _check_instance_ids(instance_ids, n=None):
+    """Host checks of a scene's instance ids: distinct integers in [0, 2^31), n of them when n is
+    given."""
+    ids = np.asarray(instance_ids).reshape(-1)
+    if ids.size and not np.issubdtype(ids.dtype, np.integer):
+        raise ValueError("instance_ids must be integers")
+    ids = ids.astype(np.int64)
+    if n is not None and len(ids) != n:
+        raise ValueError(f"{len(ids)} instance ids for {n} objects")
+    if ids.size and (ids.min() < 0 or ids.max() > np.iinfo(np.int32).max):
+        raise ValueError("instance ids must be in [0, 2^31)")
+    if len(np.unique(ids)) != len(ids):
+        raise ValueError("instance ids must be distinct")
+    return ids.astype(np.int32)
+
+
+def _pack_cads(cads):
+    """One mesh per object, packed back to back with identical meshes stored once: (vertices
+    [V,3] float64, faces [F,3] int32 indexing the packed vertices, offsets [S+1] int64, mesh [N]
+    int32), host arrays, each mesh checked by ``_check_mesh``."""
+    keys, vs, fs, offsets, mesh, base = {}, [], [], [0], [], 0
+    for cad in cads:
+        v, fc = _check_mesh(cad.vertices, cad.faces)
+        key = (v.tobytes(), fc.tobytes())
+        if key not in keys:
+            keys[key] = len(vs)
+            vs.append(v)
+            fs.append(fc + base)
+            base += len(v)
+            offsets.append(offsets[-1] + len(fc))
+        mesh.append(keys[key])
+    if not vs:                                # no object: one empty mesh keeps S >= 1
+        vs, fs, offsets = [np.zeros((0, 3))], [np.zeros((0, 3), np.int32)], [0, 0]
+    return (np.concatenate(vs), np.concatenate(fs).astype(np.int32), np.asarray(offsets, np.int64),
+            np.asarray(mesh, np.int32))
+
+
+def _render_instances_batch(vertices, faces, offsets, mesh, Ts_cad2cam, instance_ids, *, f, height,
+                            width):
+    """N <= 64 posed objects of S packed meshes rendered together into one camera
+    (csrc/render_cad.cu, mf_render_scene).  Arguments as ``_render_cad_batch``, and instance_ids
+    [N] int32, already checked on the host (``_check_instance_ids``).  Returns CUDA tensors depth
+    [H,W] float32 (NaN where nothing covers), ins [H,W] int32 (-1 where nothing covers), whole
+    [N] int32 (the pixels each object covers alone) and occluded [N,N] int32 (occluded[i, j]: the
+    pixels of object i's whole mask where object j is visible).  Four launches, no host read."""
+    import torch
+    from .. import _lib
+    from ..functions.geometry import _util
+    _lib.require_cuda(vertices, faces)
+    dev = vertices.device
+    offsets = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1))
+    d_mesh = _util.h2d_transient(np.asarray(mesh, np.int32).reshape(-1), dev, torch.int32)
+    d_ids = _util.h2d_transient(np.asarray(instance_ids, np.int32).reshape(-1), dev, torch.int32)
+    d_T = _util.h2d(Ts_cad2cam, dev, torch.float64, "render_instances/T").contiguous()
+    N = d_mesh.numel()
+    if N > MAX_SCENE_OBJECTS:
+        raise ValueError(f"at most {MAX_SCENE_OBJECTS} objects per scene, got {N}")
+    if tuple(d_T.shape) != (N, 4, 4) or d_ids.numel() != N:
+        raise ValueError("Ts_cad2cam must be [N,4,4] with one mesh index and instance id per pose")
+    H, W = int(height), int(width)
+    depth = torch.empty((H, W), dtype=torch.float32, device=dev)
+    ins = torch.empty((H, W), dtype=torch.int32, device=dev)
+    whole = torch.empty(N, dtype=torch.int32, device=dev)
+    occluded = torch.empty((N, N), dtype=torch.int32, device=dev)
+    L = _lib.lib()
+    F = faces.shape[0]
+    ws_bytes = L.mf_render_cad_workspace_bytes(N, F, H, W)
+    ws = _util.workspace(ws_bytes, dev) if ws_bytes else None
+    with torch.cuda.device(dev):
+        _lib.check(L.mf_render_scene(
+            _lib.ptr(vertices), vertices.shape[0], _lib.ptr(faces), F,
+            offsets.ctypes.data_as(_lib.ctypes.c_void_p), offsets.size - 1, _lib.ptr(d_mesh),
+            _lib.ptr(d_T), _lib.ptr(d_ids), N, float(f), H, W, _lib.ptr(depth), _lib.ptr(ins),
+            _lib.ptr(whole), _lib.ptr(occluded), _lib.ptr(ws), ws_bytes, _lib.stream()),
+            "render_scene")
+    return depth, ins, whole, occluded
+
+
+def render_instances(cads, Ts_cad2cam, instance_ids, *, fovy, height, width):
+    """Depth and instance image of posed objects rendered together into one camera, as the
+    picking-order node's ``_render_object_pose_array`` renders them with pybullet
+    (ros/src/morefusion_ros/nodes/select_picking_order.py:129-190).
+
+    ``cads`` holds one mesh per object, each with ``.vertices`` [V,3] and ``.faces`` [F,3] host
+    arrays (as ``get_cad`` returns them); identical meshes are uploaded once.  Ts_cad2cam [N,4,4]
+    maps each object's CAD points into the camera frame (OpenCV axes); instance_ids [N] are
+    distinct integers in [0, 2^31), at most 64 objects.  The camera and the rasterisation rules
+    are ``render_cad``'s; each pixel shows the object of smallest float32 depth, the earlier
+    object on an exact tie.
+
+    Returns (depth, ins): depth [H,W] float32, NaN where nothing covers; ins [H,W] int32, the
+    instance id of the visible object, -1 where nothing covers.  NumPy Ts_cad2cam gives NumPy
+    out; a CUDA tensor gives CUDA tensors out, with no host read."""
+    import torch
+    from .. import _lib
+    from ..functions.geometry import _util
+    cads = list(cads)
+    if len(cads) > MAX_SCENE_OBJECTS:
+        raise ValueError(f"at most {MAX_SCENE_OBJECTS} objects per scene, got {len(cads)}")
+    ids = _check_instance_ids(instance_ids, len(cads))
+    is_np = not isinstance(Ts_cad2cam, torch.Tensor)
+    if is_np:
+        Ts = np.asarray(Ts_cad2cam, np.float64).reshape(-1, 4, 4)
+        dev = torch.device("cuda", torch.cuda.current_device())
+    else:
+        _lib.require_cuda(Ts_cad2cam)
+        Ts = Ts_cad2cam.to(torch.float64).reshape(-1, 4, 4).contiguous()
+        dev = Ts.device
+    f = focal_from_fovy(fovy, int(height))
+    if not (np.isfinite(f) and f > 0):
+        raise ValueError("fovy must be in (0, 180) degrees")
+    v, fc, offsets, mesh = _pack_cads(cads)
+    depth, ins, _, _ = _render_instances_batch(
+        _util.h2d_transient(v, dev, torch.float64), _util.h2d_transient(fc, dev, torch.int32),
+        offsets, mesh, Ts, ids, f=f, height=height, width=width)
+    if is_np:
+        return depth.cpu().numpy(), ins.cpu().numpy()
+    return depth, ins
