@@ -1094,6 +1094,42 @@ int mf_render_scene(const double* vertices, int V, const int32_t* faces, int F,
                     float* depth, int32_t* ins, int32_t* whole, int32_t* occluded,
                     void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Model data from CAD meshes (datasets.MeshModels; what YCBVideoModels derives with binvox and
+ * trimesh, datasets/ycb_video/models.py:56-115; oracle/mesh_models.py states the rules).
+ * Meshes are packed as for mf_render_cad: vertices [V,3] f64 and faces [F,3] int32 on the
+ * device, offsets [S+1] int64 on the HOST (1 <= S <= MF_MESH_MODELS_MAX_MESHES).  Face indices
+ * must lie in [0, V) (the binding checks them on the host).
+ * mf_mesh_voxelize_solid: the D^3 solid grid of every mesh (1 <= D <= MF_MESH_MODELS_MAX_DIM):
+ *     translate [S,3], scale [S] (largest extent of the referenced vertices) and pitch [S]
+ *     (scale / D); matrix [S,D,D,D] u8 0/1 (i along x), filled when a face overlaps the voxel's
+ *     closed box or the voxel centre is inside by +z ray parity; counts [S] int32; points
+ *     [S,D^3,3] f64, mesh s's filled centres in ascending (i, j, k) in its first counts[s] rows
+ *     and NaN in the rest.  A mesh without faces, or with a zero or non-finite extent, has pitch
+ *     0 and an empty grid.  Seven launches, no host read; outputs are bitwise identical between
+ *     runs.  workspace: mf_mesh_voxelize_workspace_bytes(S, D) bytes, no initial contents.
+ * mf_mesh_signed_distance: points [P,3] f64 and mesh [P] int32 on the device.  Writes sdf [P] f64
+ *     (the distance to the nearest face of the point's mesh, positive inside by the +z parity
+ *     rule) and face [P] int32 (that face, the lowest index on a tie).  A point whose mesh is
+ *     outside [0, S), or that has a non-finite coordinate, gets NaN and -1.  Two launches, no
+ *     host read; bitwise identical between runs and to per-mesh calls.  workspace:
+ *     mf_mesh_signed_distance_workspace_bytes(P, f_max) bytes (f_max: the largest mesh's face
+ *     count), no initial contents.
+ * Both return MF_E_BADARG, before any launch, for bad offsets, sizes or NULL pointers.
+ * ------------------------------------------------------------------------ */
+#define MF_MESH_MODELS_MAX_MESHES 64
+#define MF_MESH_MODELS_MAX_DIM 128
+size_t mf_mesh_voxelize_workspace_bytes(int S, int D);
+int mf_mesh_voxelize_solid(const double* vertices, int V, const int32_t* faces, int F,
+                           const int64_t* offsets, int S, int D, uint8_t* matrix, int32_t* counts,
+                           double* points, double* translate, double* scale, double* pitch,
+                           void* workspace, size_t workspace_bytes, void* stream);
+size_t mf_mesh_signed_distance_workspace_bytes(int P, int f_max);
+int mf_mesh_signed_distance(const double* vertices, int V, const int32_t* faces, int F,
+                            const int64_t* offsets, int S, const double* points,
+                            const int32_t* mesh, int P, double* sdf, int32_t* face,
+                            void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -164,6 +164,12 @@ SIGNATURES = {
                             c_p, c_p, c_sz, c_p]),
     "mf_render_scene": (c_i, [c_p, c_i, c_p, c_i, c_p, c_i, c_p, c_p, c_p, c_i, c_d, c_i, c_i, c_p,
                               c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "mf_mesh_voxelize_workspace_bytes": (c_sz, [c_i, c_i]),
+    "mf_mesh_voxelize_solid": (c_i, [c_p, c_i, c_p, c_i, c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p,
+                                     c_p, c_sz, c_p]),
+    "mf_mesh_signed_distance_workspace_bytes": (c_sz, [c_i, c_i]),
+    "mf_mesh_signed_distance": (c_i, [c_p, c_i, c_p, c_i, c_p, c_i, c_p, c_p, c_i, c_p, c_p, c_p,
+                                      c_sz, c_p]),
 }
 
 _lib = None

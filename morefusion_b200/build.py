@@ -48,6 +48,7 @@ SOURCES = {
     "pose_metrics.cu": ["-fmad=false"],
     "training_examples.cu": ["-fmad=false"],
     "render_cad.cu": ["-fmad=false"],
+    "mesh_models.cu": ["-fmad=false"],
 }
 
 

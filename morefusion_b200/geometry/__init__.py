@@ -477,3 +477,177 @@ def render_instances(cads, Ts_cad2cam, instance_ids, *, fovy, height, width):
     if is_np:
         return depth.cpu().numpy(), ins.cpu().numpy()
     return depth, ins
+
+
+MAX_MODEL_MESHES = 64                     # MF_MESH_MODELS_MAX_MESHES
+MAX_GRID_DIMENSION = 128                  # MF_MESH_MODELS_MAX_DIM
+
+
+def _check_model_mesh(vertices, faces):
+    """``_check_mesh`` plus what the model data needs: at least one face, finite vertices and a
+    non-zero extent of the referenced vertices."""
+    v, fc = _check_mesh(vertices, faces)
+    if len(fc) == 0:
+        raise ValueError("the mesh has no faces")
+    used = v[fc.reshape(-1)]
+    if not np.isfinite(v).all():
+        raise ValueError("vertices must be finite")
+    if not (used.max(0) - used.min(0)).max() > 0:
+        raise ValueError("the mesh's referenced vertices span no extent")
+    return v, fc
+
+
+def _pack_meshes(meshes):
+    """(vertices, faces) pairs checked by ``_check_model_mesh`` and packed back to back: (vertices
+    [V,3] float64, faces [F,3] int32 indexing the packed vertices, offsets [S+1] int64)."""
+    vs, fs, offsets, base = [], [], [0], 0
+    for v, fc in meshes:
+        v, fc = _check_model_mesh(v, fc)
+        vs.append(v)
+        fs.append(fc + base)
+        base += len(v)
+        offsets.append(offsets[-1] + len(fc))
+    if not 1 <= len(vs) <= MAX_MODEL_MESHES:
+        raise ValueError(f"1 to {MAX_MODEL_MESHES} meshes per call, got {len(vs)}")
+    return np.concatenate(vs), np.concatenate(fs).astype(np.int32), np.asarray(offsets, np.int64)
+
+
+def _voxelize_solid_batch(vertices, faces, offsets, dimension):
+    """The solid grids of S packed meshes (csrc/mesh_models.cu, mf_mesh_voxelize_solid): vertices
+    [V,3] float64 and faces [F,3] int32 CUDA tensors checked on the host, offsets [S+1] host
+    int64.  Returns CUDA tensors matrix [S,D,D,D] bool, counts [S] int32, points [S,D^3,3]
+    float64 (mesh s's filled centres in its first counts[s] rows, NaN after), translate [S,3],
+    scale [S] and pitch [S] float64.  Seven launches, no host read."""
+    import torch
+    from .. import _lib
+    from ..functions.geometry import _util
+    _lib.require_cuda(vertices, faces)
+    D = int(dimension)
+    if not 1 <= D <= MAX_GRID_DIMENSION:
+        raise ValueError(f"dimension must be in [1, {MAX_GRID_DIMENSION}], got {dimension}")
+    dev = vertices.device
+    offsets = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1))
+    S = offsets.size - 1
+    matrix = torch.empty((S, D, D, D), dtype=torch.bool, device=dev)
+    counts = torch.empty(S, dtype=torch.int32, device=dev)
+    points = torch.empty((S, D ** 3, 3), dtype=torch.float64, device=dev)
+    translate = torch.empty((S, 3), dtype=torch.float64, device=dev)
+    scale = torch.empty(S, dtype=torch.float64, device=dev)
+    pitch = torch.empty(S, dtype=torch.float64, device=dev)
+    L = _lib.lib()
+    ws_bytes = L.mf_mesh_voxelize_workspace_bytes(S, D)
+    ws = _util.workspace(ws_bytes, dev)
+    with torch.cuda.device(dev):
+        _lib.check(L.mf_mesh_voxelize_solid(
+            _lib.ptr(vertices), vertices.shape[0], _lib.ptr(faces), faces.shape[0],
+            offsets.ctypes.data_as(_lib.ctypes.c_void_p), S, D, _lib.ptr(matrix.view(torch.uint8)),
+            _lib.ptr(counts), _lib.ptr(points), _lib.ptr(translate), _lib.ptr(scale),
+            _lib.ptr(pitch), _lib.ptr(ws), ws_bytes, _lib.stream()), "voxelize_solid")
+    return matrix, counts, points, translate, scale, pitch
+
+
+def _signed_distance_batch(vertices, faces, offsets, points, mesh):
+    """Signed distances of points [P,3] float64 (CUDA) to S packed meshes (csrc/mesh_models.cu,
+    mf_mesh_signed_distance); mesh [P] int32 CUDA, the mesh of each point (a point outside [0, S)
+    gets NaN and -1).  Returns CUDA tensors sdf [P] float64 (positive inside) and face [P] int32
+    (the nearest face, an index into the packed faces).  Two launches, no host read."""
+    import torch
+    from .. import _lib
+    from ..functions.geometry import _util
+    _lib.require_cuda(vertices, faces, points, mesh)
+    dev = vertices.device
+    offsets = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1))
+    points = points.to(torch.float64).reshape(-1, 3).contiguous()
+    mesh = mesh.to(torch.int32).reshape(-1).contiguous()
+    P = points.shape[0]
+    if mesh.numel() != P:
+        raise ValueError("one mesh index per point")
+    sdf = torch.empty(P, dtype=torch.float64, device=dev)
+    face = torch.empty(P, dtype=torch.int32, device=dev)
+    if P == 0:
+        return sdf, face
+    L = _lib.lib()
+    f_max = int(np.diff(offsets).max())
+    with torch.cuda.device(dev):
+        ws_bytes = L.mf_mesh_signed_distance_workspace_bytes(P, f_max)
+        ws = _util.workspace(ws_bytes, dev)
+        _lib.check(L.mf_mesh_signed_distance(
+            _lib.ptr(vertices), vertices.shape[0], _lib.ptr(faces), faces.shape[0],
+            offsets.ctypes.data_as(_lib.ctypes.c_void_p), offsets.size - 1, _lib.ptr(points),
+            _lib.ptr(mesh), P, _lib.ptr(sdf), _lib.ptr(face), _lib.ptr(ws), ws_bytes,
+            _lib.stream()), "signed_distance")
+    return sdf, face
+
+
+def _host_mesh(vertices, faces):
+    """Host copies of a mesh given as NumPy or CUDA tensors, and the device to run on."""
+    import torch
+    from .. import _lib
+    if isinstance(vertices, torch.Tensor):
+        _lib.require_cuda(vertices)
+        dev = vertices.device
+        v = vertices.detach().cpu().numpy()
+    else:
+        dev = torch.device("cuda", torch.cuda.current_device())
+        v = vertices
+    fc = faces.detach().cpu().numpy() if isinstance(faces, torch.Tensor) else faces
+    return v, fc, dev
+
+
+def voxelize_solid(vertices, faces, dimension=64):
+    """The solid D^3 voxel grid of a mesh, as YCBVideoModels.get_solid_voxel_grid gets it from
+    ``binvox -d 64`` (datasets/ycb_video/models.py:81-86), by the rules of DESIGN section 4.22:
+    the grid spans the referenced vertices' bounding box from its minimum corner, with cubic
+    voxels of side scale / D (scale: the largest extent); a voxel is filled when a face overlaps
+    its closed box or its centre is inside by +z ray parity.  The winding need not be consistent.
+
+    Returns an object with ``.matrix`` [D,D,D] bool (i along x), ``.points`` [n,3] float64 (the
+    filled voxel centres in ascending (i, j, k)), ``.translate`` [3] (the grid's minimum corner),
+    ``.pitch`` (the voxel side) and ``.scale`` (floats).  NumPy in gives NumPy out; CUDA tensors
+    in give CUDA tensors out, after one host read (the number of points).  ValueError, before any
+    launch, for a mesh without faces, face indices outside [0, V), non-finite vertices, a zero
+    extent or a dimension outside [1, 128]."""
+    import types
+    import torch
+    from ..functions.geometry import _util
+    is_np = not isinstance(vertices, torch.Tensor)
+    v, fc, dev = _host_mesh(vertices, faces)
+    v, fc = _check_model_mesh(v, fc)
+    matrix, counts, points, translate, scale, pitch = _voxelize_solid_batch(
+        _util.h2d_transient(v, dev, torch.float64), _util.h2d_transient(fc, dev, torch.int32),
+        [0, len(fc)], dimension)
+    head = torch.cat([counts.to(torch.float64), scale, pitch]).cpu().numpy()
+    n = int(head[0])
+    out = types.SimpleNamespace(matrix=matrix[0], points=points[0, :n], translate=translate[0],
+                                scale=float(head[1]), pitch=float(head[2]))
+    if is_np:
+        out.matrix = out.matrix.cpu().numpy()
+        out.points = out.points.cpu().numpy()
+        out.translate = out.translate.cpu().numpy()
+    return out
+
+
+def signed_distance(vertices, faces, points):
+    """Signed distance of points [P,3] to a mesh, as trimesh's ``nearest.signed_distance``
+    gives it to YCBVideoModels._get_sdf (datasets/ycb_video/models.py:77): the distance to the
+    closest point of the nearest face, positive inside.  Inside is the +z ray parity rule of
+    ``voxelize_solid``, so the grid and the sign agree.  Returns sdf [P] float64.  NumPy in gives
+    NumPy out; CUDA tensors in give CUDA tensors out, with no host read besides the face check.
+    ValueError, before any launch, as ``voxelize_solid``."""
+    import torch
+    from .. import _lib
+    from ..functions.geometry import _util
+    is_np = not isinstance(points, torch.Tensor)
+    v, fc, dev = _host_mesh(vertices, faces)
+    v, fc = _check_model_mesh(v, fc)
+    if is_np:
+        p = np.asarray(points, np.float64).reshape(-1, 3)
+        d_p = _util.h2d_transient(p, dev, torch.float64)
+    else:
+        _lib.require_cuda(points)
+        d_p = points.to(torch.float64).reshape(-1, 3).contiguous()
+    mesh = torch.zeros(d_p.shape[0], dtype=torch.int32, device=dev)
+    sdf, _ = _signed_distance_batch(_util.h2d_transient(v, dev, torch.float64),
+                                    _util.h2d_transient(fc, dev, torch.int32), [0, len(fc)], d_p,
+                                    mesh)
+    return sdf.cpu().numpy() if is_np else sdf
