@@ -883,6 +883,10 @@ int mf_average_distance_bwd_batched(const float* gout, const float* points, int 
  *     voxel_size); writes one row per occupied voxel in ascending (i, j, k) at means[m*N ...]
  *     [*,3] f64 (the mean of its points, summed in row order), keys [*,3] int32, counts [*] int32,
  *     and n_out[m], the number of voxels (<= the cloud's finite rows, so nothing can overflow).
+ *     A cloud whose keys reach 2^31 - 1 on an axis is refused, n_out[m] = -1 and no row written,
+ *     rather than having voxels merged at the int32 limit; mf_icp_cell_list refuses such a cloud
+ *     with a NaN origin, and mf_icp_run gives an instance with a refused source or target NaN
+ *     transform, fitness and rmse and 0 iterations.
  *     One CTA per cloud; deterministic.  workspace: mf_icp_sort_workspace_bytes(M, N).
  * mf_icp_cell_list: a uniform cell list of side cell_size over the first *n_points rows of one
  *     float64 cloud [N,3] (the down-sampled CAD cloud): the rows sorted by cell (i, j, k)

@@ -45,7 +45,8 @@ def voxel_down_sample(points, voxel_size):
     """Open3D's ``voxel_down_sample`` of M clouds at once.  points: CUDA [M,N,3] (or [M,H,W,3])
     float32 / float64; rows with a non-finite coordinate are skipped.  Returns CUDA tensors
     (means [M,N,3] float64, keys [M,N,3] int32, counts [M,N] int32, n [M] int32): cloud m's n[m]
-    voxels are its first rows, in ascending (i, j, k)."""
+    voxels are its first rows, in ascending (i, j, k).  n[m] = -1 refuses a cloud that spans
+    2^31 - 1 voxels or more on an axis, whose keys would not fit in int32."""
     pts = _points(points)
     _lib.require_cuda(pts)
     M, N = pts.shape[0], pts.shape[1]
@@ -109,7 +110,9 @@ def register_batch(source, targets, transform_init, *, voxel_size=VOXEL_SIZE, ma
     2 * voxel_size and must equal each target's.
 
     Returns CUDA tensors (transform [M,4,4] float64, fitness [M], inlier_rmse [M] float64,
-    iterations [M] int32).  No host read."""
+    iterations [M] int32).  No host read.  An instance whose source or target spans 2^31 - 1
+    voxels (or target cells) or more on an axis is refused: NaN transform, fitness and rmse, 0
+    iterations."""
     src = _points(source)
     _lib.require_cuda(src)
     M, N = src.shape[0], src.shape[1]
@@ -165,6 +168,8 @@ class ICPRegistration:
         T, fit, rmse, _ = register_batch(src, [tgt], init[None], voxel_size=voxel_size,
                                          max_iteration=iteration)
         out = torch.cat([T.reshape(-1), fit, rmse]).cpu().numpy()
+        if not np.isfinite(out).all():
+            raise ValueError("a cloud spans 2^31 - 1 voxels or more on an axis")
         return np.linalg.inv(out[:16].reshape(4, 4)), float(out[16]), float(out[17])
 
     def register(self, iteration=None, voxel_size=None):

@@ -3,12 +3,19 @@
 // list over the CAD cloud, and every iteration of every instance in one launch.
 //
 // Built with -fmad=false: the voxel keys, the down-sampled means and the d^2 threshold tests are
-// the oracle's float64 expressions, rounded step by step.
+// the oracle's float64 expressions, rounded step by step.  With g++ -DMF_HOST_EMU (and
+// -ffp-contract=off) only the per-thread helpers compile: cell_window, nearest, horn_rotation and
+// apply, which tests/emu/icp_emu.cpp runs on the host.
 #include <float.h>
 #include <limits.h>
 #include <math.h>
 
+#ifdef MF_HOST_EMU
+#include "mapping_emu_stubs.h"
+#include "../../include/morefusion_b200.h"
+#else
 #include "common.cuh"
+#endif
 
 namespace {
 
@@ -22,13 +29,28 @@ template <typename T>
 __device__ __forceinline__ double ld(const T* p, long long i) { return (double)p[i]; }
 
 // floor((x - origin) / size) clamped to [0, INT_MAX]: a key below 0 cannot occur for a point of
-// the cloud itself; the clamp keeps a far query's window representable
+// the cloud itself.  A point's key is INT_MAX only when it does not fit (KEY_MAX below): the
+// cloud is then refused rather than having distinct voxels merged at the clamp.
 __device__ __forceinline__ int cell_of(double x, double origin, double size) {
   double c = floor((x - origin) / size);
   if (!(c > 0.0)) return 0;
   if (c >= (double)INT_MAX) return INT_MAX;
   return (int)c;
 }
+
+constexpr int KEY_MAX = INT_MAX - 1;        // the largest key a sorted cloud holds
+
+// The cells [*lo, *hi] on one axis that can hold a point within r of x: those of x - r and x + r,
+// both capped at KEY_MAX.  No key of a cell list exceeds KEY_MAX, so the cap drops no candidate,
+// and a loop `for (c = lo; c <= hi; ++c)` ends: with hi = INT_MAX, ++c would overflow instead
+// (a query at origin + (2^31 - 1) h or beyond, e.g. an init 1e8 m off at h = 2 cm).
+__device__ __forceinline__ void cell_window(double x, double r, double origin, double h, int* lo,
+                                            int* hi) {
+  *lo = min(cell_of(x - r, origin, h), KEY_MAX);
+  *hi = min(cell_of(x + r, origin, h), KEY_MAX);
+}
+
+#ifndef MF_HOST_EMU
 
 __device__ __forceinline__ int axis(int4 v, int a) { return a == 0 ? v.x : (a == 1 ? v.y : v.z); }
 
@@ -138,6 +160,13 @@ k_icp_sort(const T* __restrict__ points, int N, const int32_t* __restrict__ n_ro
     int v = 0;
     for (int i = 0; i < SORT_WARPS; ++i) v = max(v, s_ired[i][a]);
     kmax[a] = v;
+  }
+  // a key past KEY_MAX does not fit in int32: refuse the cloud (n_out = -1, or a NaN origin)
+  // rather than merge the voxels beyond it; k_icp_run refuses such a source or target in turn
+  if (kmax[0] > KEY_MAX || kmax[1] > KEY_MAX || kmax[2] > KEY_MAX) {
+    if (CELLS && tid < 3) out_origin[3 * m + tid] = nan("");
+    if (!CELLS && tid == 0) n_out[m] = -1;
+    return;
   }
 
   // each warp owns a contiguous chunk, so a digit's items keep their order: the sort is stable
@@ -291,6 +320,8 @@ __device__ void block_sum(double* v, double (*s)[K], double* s_out) {
   __syncthreads();
 }
 
+#endif  // !MF_HOST_EMU
+
 __device__ __forceinline__ void apply(const double* T, double& x, double& y, double& z) {
   const double a = ((T[0] * x + T[1] * y) + T[2] * z) + T[3];
   const double b = ((T[4] * x + T[5] * y) + T[6] * z) + T[7];
@@ -304,10 +335,11 @@ __device__ __forceinline__ void apply(const double* T, double& x, double& y, dou
 // search over the cell list is exact.
 __device__ int nearest(double qx, double qy, double qz, const mf_icp_target& tg, int nt, double r,
                        double r2, double* d2_out) {
-  const double ox = tg.origin[0], oy = tg.origin[1], oz = tg.origin[2], h = tg.cell_size;
-  const int i0 = cell_of(qx - r, ox, h), i1 = cell_of(qx + r, ox, h);
-  const int j0 = cell_of(qy - r, oy, h), j1 = cell_of(qy + r, oy, h);
-  const int k0 = cell_of(qz - r, oz, h), k1 = cell_of(qz + r, oz, h);
+  const double h = tg.cell_size;
+  int i0, i1, j0, j1, k0, k1;
+  cell_window(qx, r, tg.origin[0], h, &i0, &i1);
+  cell_window(qy, r, tg.origin[1], h, &j0, &j1);
+  cell_window(qz, r, tg.origin[2], h, &k0, &k1);
   const int* C = tg.cells;
   double best = r2;
   int bi = -1, bidx = INT_MAX;
@@ -402,6 +434,8 @@ __device__ void horn_rotation(const double* C, double* R) {
   R[6] = 2.0 * (x * z - w * y); R[7] = 2.0 * (y * z + w * x); R[8] = 1.0 - 2.0 * (x * x + y * y);
 }
 
+#ifndef MF_HOST_EMU
+
 // One CTA per instance: Open3D's RegistrationICP loop (oracle/icp.py) from init to convergence
 // or max_iteration, the source points resident in shared memory when they fit (else in `work`).
 __global__ void __launch_bounds__(RUN_THREADS)
@@ -423,6 +457,17 @@ k_icp_run(const double* __restrict__ source, int N, const int32_t* __restrict__ 
   const mf_icp_target tg = targets[m];
   const int nt = *tg.count;
   const double r2 = r * r;
+  // a source or target cloud k_icp_sort refused (a key past KEY_MAX): NaN out, no iteration
+  if (n_source[m] < 0 || nt < 0 ||
+      !(isfinite(tg.origin[0]) && isfinite(tg.origin[1]) && isfinite(tg.origin[2]))) {
+    if (tid < 16) out_T[16 * m + tid] = nan("");
+    if (tid == 0) {
+      out_fitness[m] = nan("");
+      out_rmse[m] = nan("");
+      out_iterations[m] = 0;
+    }
+    return;
+  }
   if (tid < 16) s_T[tid] = init[16 * m + tid];
   __syncthreads();
   for (int i = tid; i < n; i += RUN_THREADS) {
@@ -521,8 +566,11 @@ k_icp_run(const double* __restrict__ source, int N, const int32_t* __restrict__ 
 
 size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
+#endif  // !MF_HOST_EMU
+
 }  // namespace
 
+#ifndef MF_HOST_EMU
 extern "C" size_t mf_icp_sort_workspace_bytes(int M, int N) {
   if (M < 0 || N < 0) return 0;
   return 2 * align256((size_t)M * N * sizeof(int4));
@@ -610,3 +658,4 @@ extern "C" int mf_icp_run(int M, const double* source, int N, const int32_t* n_s
   MF_LAUNCH_CHECK();
   return MF_OK;
 }
+#endif  // !MF_HOST_EMU

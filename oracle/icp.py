@@ -23,7 +23,8 @@ Eigen's ``umeyama``) rather than running it:
 Rank of sigma: with one correspondence sigma is exactly 0 and the update is a pure translation
 (U = V = I).  The kernel shares that rule (csrc/icp.cu).  With sigma of rank 1 (two, or collinear,
 correspondences) the rotation is not determined by the matches; neither the kernel nor this
-restatement is pinned to Eigen's choice there, and the tests do not exercise it.
+restatement is pinned to Eigen's choice there.  The tests check the kernel's rotation there by
+its properties instead: a proper rotation that attains the maximum of tr(R^T sigma).
 """
 
 import numpy as np
@@ -69,6 +70,10 @@ def correspondences(source, target, max_distance):
     t = np.asarray(target, np.float64)
     if len(s) == 0 or len(t) == 0:
         return (np.full(len(s), -1, np.int64), np.full(len(s), np.inf), np.full(len(s), np.inf))
+    step = max(1, (1 << 24) // len(t))                 # rows per block: memory stays bounded
+    if len(s) > step:
+        parts = [correspondences(s[i:i + step], t, max_distance) for i in range(0, len(s), step)]
+        return tuple(np.concatenate(x) for x in zip(*parts))
     dx = s[:, None, 0] - t[None, :, 0]
     dy = s[:, None, 1] - t[None, :, 1]
     dz = s[:, None, 2] - t[None, :, 2]
@@ -84,6 +89,20 @@ def correspondences(source, target, max_distance):
     return match, best, gap
 
 
+def umeyama_rotation(sigma, det_correction=True):
+    """Umeyama's rotation of the cross-covariance sigma [3,3] = sum (t - t_mean)(s - s_mean)^T / n:
+    R = U S V^T with S[2] = -1 when det(U) det(V) < 0; I for sigma = 0.  det_correction=False
+    drops the S[2] rule (a wrong reference for the tests: it can return a reflection)."""
+    sigma = np.asarray(sigma, np.float64)
+    if not sigma.any():
+        return np.eye(3)
+    U, _, Vt = np.linalg.svd(sigma)
+    S = np.ones(3)
+    if det_correction and np.linalg.det(U) * np.linalg.det(Vt) < 0:
+        S[2] = -1.0
+    return U @ np.diag(S) @ Vt
+
+
 def umeyama(src, dst):
     """Eigen::umeyama(src^T, dst^T, false) in float64: the rigid [4,4] with dst ~ R src + t."""
     T = np.eye(4)
@@ -92,14 +111,7 @@ def umeyama(src, dst):
         return T
     sm, dm = src.mean(0), dst.mean(0)
     sigma = (dst - dm).T @ (src - sm) / n
-    if not sigma.any():
-        R = np.eye(3)
-    else:
-        U, _, Vt = np.linalg.svd(sigma)
-        S = np.ones(3)
-        if np.linalg.det(U) * np.linalg.det(Vt) < 0:
-            S[2] = -1.0
-        R = U @ np.diag(S) @ Vt
+    R = umeyama_rotation(sigma)
     T[:3, :3] = R
     T[:3, 3] = dm - R @ sm
     return T
